@@ -403,27 +403,31 @@ int run_row_pass(const avirb200_plan* pl, const void* d_src, size_t src_pitch, f
         if (r == -1) return fail(AVIRB200_ERR_CUDA, "fast row pass launch failed");
         if (r == 0) { ++*launches; return 0; }
     }
-    if (p4) return fail(AVIRB200_ERR_UNSUPPORTED, "row pass: the 4-channel kernels could not take this band");
+    // The generic kernel.  Its intermediate rows are dst_w * mid_ch floats apart, as every other
+    // kernel family and every band / halo offset lays them out.  A widened band the 4-channel kernels
+    // did not take runs it on the widened copy with 4 channels (the pad channel's results are dropped).
     PassParams p;
     std::memset(&p, 0, sizeof p);
     fill_common(p, pl);
+    const PassConfig c = p4 ? choose_generic_config(pl->h.hostdev, 4, 0, d.dst_w) : pl->cfg_h;
+    if (p4) p.channels = 4;
     p.ax = pl->h.dev;
     p.is_v = 0;
     p.n_lines = rows;
-    p.lines_per_block = pl->cfg_h.lines_per_block;
-    p.tile_out = pl->cfg_h.tile_out;
+    p.lines_per_block = c.lines_per_block;
+    p.tile_out = c.tile_out;
     p.out0 = 0;
     p.out1 = d.dst_w;
-    p.span = pl->cfg_h.span;
-    p.pitch = pl->cfg_h.pitch;
+    p.span = c.span;
+    p.pitch = c.pitch;
     p.src = d_src;
     p.src_pitch = (long long)src_pitch;
     p.src_type = d.in_type;
     p.dst = d_mid;
-    p.dst_pitch = (long long)d.dst_w * d.channels;
+    p.dst_pitch = (long long)d.dst_w * pl->mid_ch;
     p.dst_type = AVIRB200_F32;
     ++*launches;
-    return launch_generic(p, pl->cfg_h, st);
+    return launch_generic(p, c, st);
 }
 
 // scratch4: where the band's 4-channel destination rows go when use_pad4(pl) (then narrowed into d_dst).
@@ -487,15 +491,18 @@ int run_col_pass(const avirb200_plan* pl, const float* d_mid, int mid_row_base, 
         if (r == -1) return fail(AVIRB200_ERR_CUDA, "fast column pass launch failed");
         if (r == 0) { ++*launches; return finish(); }
     }
-    if (p4) return fail(AVIRB200_ERR_UNSUPPORTED, "column pass: the 4-channel kernels could not take this band");
+    // The generic kernel (intermediate rows dst_w * mid_ch floats apart, see run_row_pass).  A widened
+    // band the tile kernel refused (a shard whose footprint exceeds its shared memory) runs it with 4
+    // channels into the 4-channel scratch, narrowed as after the 4-channel kernels.
     PassParams p;
     std::memset(&p, 0, sizeof p);
     fill_common(p, pl);
+    if (p4) p.channels = 4;
     p.ax = pl->v.dev;
     p.is_v = 1;
     p.n_lines = d.dst_w;
     PassConfig c = pl->cfg_v;
-    if (out0 != 0 || out1 != d.dst_h) c = choose_generic_config(pl->v.hostdev, d.channels, out0, out1);
+    if (p4 || out0 != 0 || out1 != d.dst_h) c = choose_generic_config(pl->v.hostdev, p.channels, out0, out1);
     p.lines_per_block = c.lines_per_block;
     p.tile_out = c.tile_out;
     p.out0 = out0;
@@ -503,7 +510,7 @@ int run_col_pass(const avirb200_plan* pl, const float* d_mid, int mid_row_base, 
     p.span = c.span;
     p.pitch = c.pitch;
     p.src = d_mid;
-    p.src_pitch = (long long)d.dst_w * d.channels;
+    p.src_pitch = (long long)d.dst_w * pl->mid_ch;
     p.src_type = AVIRB200_F32;
     p.src_row_base = mid_row_base;
     p.dst = d_dst;
@@ -511,7 +518,8 @@ int run_col_pass(const avirb200_plan* pl, const float* d_mid, int mid_row_base, 
     p.dst_type = d.out_type;
     p.dst_row_base = out0;
     ++*launches;
-    return launch_generic(p, c, st);
+    const int r = launch_generic(p, c, st);
+    return r != 0 ? r : finish();
 }
 
 // ---- NCCL through dlopen (no link-time dependency) -------------------------------------------

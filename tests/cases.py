@@ -174,6 +174,83 @@ def count_mismatch(a, b):
     return int((a != b).sum())
 
 
+# ---- caller layouts: padded pitches, offset bases, poisoned padding, guarded destinations ------------
+
+SENTINEL = 0xA5  # every guard byte of a destination buffer
+GUARD_ROWS = 2   # guard rows above and below a destination image
+
+
+def poison_of(dtype):
+    """Fill of a source buffer outside the image: a value no kernel may let into a result."""
+    dtype = np.dtype(dtype)
+    return np.nan if dtype.kind == "f" else np.iinfo(dtype).max
+
+
+def image_view(backing, origin, pitch, shape):
+    """(H, W, C) view of `backing` (1-D) starting at element `origin`, rows `pitch` elements apart."""
+    h, w, c = shape
+    it = backing.dtype.itemsize
+    return np.lib.stride_tricks.as_strided(backing[origin:], shape=(h, w, c), strides=(pitch * it, c * it, it))
+
+
+def host_array(n, dtype, pinned=False):
+    """n elements of pageable (numpy) or page-locked (torch pin_memory) host memory."""
+    dtype = np.dtype(dtype)
+    if not pinned:
+        return np.empty(n, dtype)
+    import torch
+    return torch.empty(n * dtype.itemsize, dtype=torch.uint8).pin_memory().numpy().view(dtype)
+
+
+class Layout:
+    """An image inside a larger 1-D buffer: `origin` (elements) of pixel (0, 0), `pitch` (elements)
+    from one row to the next.  view() is the (H, W, C) image, is_outside() marks every byte of
+    the buffer that is not part of it."""
+
+    def __init__(self, backing, origin, pitch, shape):
+        self.backing, self.origin, self.pitch, self.shape = backing, origin, pitch, tuple(shape)
+
+    def view(self, backing=None):
+        return image_view(self.backing if backing is None else backing, self.origin, self.pitch, self.shape)
+
+    def outside_bytes(self, backing=None):
+        """The bytes of (a copy of) the buffer outside the image, as a flat uint8 array."""
+        b = (self.backing if backing is None else backing).view(np.uint8)
+        inside = np.zeros(b.size, bool)
+        h, w, c = self.shape
+        it = self.backing.dtype.itemsize
+        image_view(inside, self.origin * it, self.pitch * it, (h, w * c * it, 1))[:] = True
+        return b[~inside]
+
+
+def source_layout(img, extra_pitch=0, elem_offset=0, pinned=False):
+    """`img` copied into a buffer with rows sw*C + extra_pitch elements apart, starting elem_offset
+    elements in; every element outside the image holds poison_of(dtype)."""
+    h, w, c = img.shape
+    pitch = w * c + extra_pitch
+    back = host_array(elem_offset + h * pitch + extra_pitch + 8, img.dtype, pinned)
+    back[:] = poison_of(img.dtype)
+    lay = Layout(back, elem_offset, pitch, img.shape)
+    lay.view()[:] = img
+    return lay
+
+
+def guarded_dest(shape, dtype, extra_pitch=0, elem_offset=0, pinned=False):
+    """A destination buffer for an (H, W, C) image: GUARD_ROWS rows above and below, rows
+    W*C + extra_pitch elements apart, the image elem_offset elements into its row; every byte
+    set to SENTINEL."""
+    h, w, c = shape
+    pitch = w * c + extra_pitch
+    back = host_array((h + 2 * GUARD_ROWS) * pitch + elem_offset + 8, dtype, pinned)
+    back.view(np.uint8)[:] = SENTINEL
+    return Layout(back, GUARD_ROWS * pitch + elem_offset, pitch, shape)
+
+
+def guard_damage(lay, backing=None):
+    """Number of bytes outside the image that no longer hold SENTINEL."""
+    return int((lay.outside_bytes(backing) != SENTINEL).sum())
+
+
 def case_id(case):
     fp, sw, sh, nw, nh, ch, ti, to, rb, kw = case
     s = "%s-%dx%d-%dx%d-c%d-%s-%s-b%d" % (("def", "f4", "dil", "defE", "f4E", "dilE")[fp], sw, sh, nw, nh, ch,

@@ -26,6 +26,9 @@ CASES = [
     (2, 1920, 2160, 480, 540, 4, u8, u8, 8, {"gamma": True, "alpha": 3}),  # cfg5 chain (tile kernel)
     (1, 960, 1080, 1920, 2160, 4, u8, u8, 8, {}),                    # cfg2: upsizing
     (0, 700, 900, 431, 557, 3, u8, u8, 8, {}),                       # generic kernel, odd ratio, RGB
+    # RGB widened onto the 4-channel kernels, both passes forced onto the generic kernel: the halo rows
+    # and band offsets of a 4-float intermediate
+    (0, 1280, 1440, 640, 720, 3, u8, u8, 8, {"family": 1}),
 ]
 
 
@@ -74,6 +77,7 @@ def main():
             plan = C.c_void_p()
             assert lib.avirb200_plan_create(C.c_void_p(dp), C.byref(plan)) == 0, lib.avirb200_last_error()
             assert lib.avirb200_plan_set_option(plan, ab.OPT_OVERLAP_HALO, overlap) == 0
+            assert lib.avirb200_plan_set_option(plan, ab.OPT_KERNEL_FAMILY, kw.get("family", 0)) == 0
             si = SI()
             assert lib.avirb200_shard_query(plan, rank, world, C.byref(si)) == 0, lib.avirb200_last_error()
             wsb, wsf = C.c_size_t(), C.c_size_t()

@@ -97,13 +97,25 @@ def fnv1a64(a):
     return "%016x" % hsh
 
 
+def _rows(a, pitch):
+    """a itself when its rows lie `pitch` elements apart with packed pixels (a strided view into a
+    padded buffer: upstream then reads that buffer), a contiguous copy when pitch < 1."""
+    if pitch < 1:
+        return np.ascontiguousarray(a)
+    it = a.dtype.itemsize
+    assert a.strides[1:] == (a.shape[2] * it, it) and (a.shape[0] < 2 or a.strides[0] == pitch * it)
+    return a
+
+
 def ref_resize(src, nw, nh, out_dtype, fpclass=FP_FLOAT4, k=0.0, resbits=8, srcbits=0,
-               ox=0.0, oy=0.0, gamma=False, alpha=-1, buildmode=-1, nthreads=1, params=0):
-    src = np.ascontiguousarray(src)
+               ox=0.0, oy=0.0, gamma=False, alpha=-1, buildmode=-1, nthreads=1, params=0,
+               src_pitch=0):
+    """Upstream resizeImage; src_pitch > 0 is its SrcScanlineSize (src a strided view, see _rows)."""
+    src = _rows(src, src_pitch)
     sh, sw, c = src.shape
     dst = np.zeros((nh, nw, c), dtype=out_dtype)
     r = ref().avir_ref_resize(fpclass, T_OF[src.dtype], T_OF[np.dtype(out_dtype)],
-                              src.ctypes.data, sw, sh, 0, dst.ctypes.data, nw, nh, c,
+                              src.ctypes.data, sw, sh, src_pitch, dst.ctypes.data, nw, nh, c,
                               k, resbits, srcbits, ox, oy, int(gamma), alpha, buildmode,
                               nthreads, params)
     assert r == 0
@@ -163,10 +175,20 @@ def parse_plan(buf):
     return plan
 
 
-def lancir_ref(src, nw, nh, out_dtype, kx=0.0, ky=0.0, ox=0.0, oy=0.0, la=3.0):
-    src = np.ascontiguousarray(src)
+def lancir_ref(src, nw, nh, out_dtype, kx=0.0, ky=0.0, ox=0.0, oy=0.0, la=3.0, srcssize=0,
+               newssize=0, dst=None):
+    """Upstream CLancIR::resizeImage.  srcssize / newssize > 0 are its SrcSSize / NewSSize: src /
+    dst are then strided views into padded buffers (dst, required with newssize, is written in
+    place and returned)."""
+    src = _rows(src, srcssize)
     sh, sw, c = src.shape
-    dst = np.zeros((nh, nw, c), dtype=out_dtype)
+    if dst is None:
+        assert newssize < 1
+        dst = np.zeros((nh, nw, c), dtype=out_dtype)
+    else:
+        dst = _rows(dst, newssize)
+        assert dst.shape == (nh, nw, c) and dst.dtype == np.dtype(out_dtype)
     r = ref().lancir_ref_resize(T_OF[src.dtype], T_OF[np.dtype(out_dtype)], src.ctypes.data,
-                                sw, sh, dst.ctypes.data, nw, nh, c, 0, 0, kx, ky, ox, oy, la)
+                                sw, sh, dst.ctypes.data, nw, nh, c, srcssize, newssize, kx, ky, ox,
+                                oy, la)
     return r, dst

@@ -147,12 +147,24 @@ def test_deselected_streaming_chains_bit_exact(case):
 
 # ---- pipelined host call: row bands over copy-in / compute / copy-out streams ----------------
 
-@pytest.mark.parametrize("bands", [2, 3, 7, 16])
-@pytest.mark.parametrize("case", [MEDIUM[0], MEDIUM[2], MEDIUM[3], MEDIUM[4], MEDIUM[6],
-                                  (0, 300, 200, 431, 287, 3, np.uint8, np.uint8, 8, {})], ids=cs.case_id)
-def test_banded_host_call_matches_single_band(case, bands):
-    """avirb200_resize_host cuts large images into row bands so that PCIe transfers overlap the
-    kernels; the band count must not change a bit (the HOST_BANDS plan option forces it)."""
+BANDED = [MEDIUM[0], MEDIUM[2], MEDIUM[3], MEDIUM[4], MEDIUM[6],
+          (0, 300, 200, 431, 287, 3, np.uint8, np.uint8, 8, {}),
+          # 1..3 channels widened onto the 4-channel kernels: an intermediate of 4 floats a pixel,
+          # whichever kernel family runs the passes
+          (0, 640, 480, 320, 240, 3, np.uint8, np.uint8, 8, {}),
+          (1, 640, 480, 320, 240, 1, np.float32, np.float32, 16, {})]
+_banded_expected = {}
+
+
+@pytest.fixture(params=[2, 1], ids=["tile", "generic"])
+def other_family(request):
+    """The kernel families other than the product order (front-end default and raw plans alike)."""
+    ab.set_option(ab.OPT_KERNEL_FAMILY, request.param)
+    yield request.param
+    ab.set_option(ab.OPT_KERNEL_FAMILY, -1)
+
+
+def _check_banded(case, bands):
     src = cs.make_input(case, seed=23)
     ab.set_option(ab.OPT_HOST_BANDS, 1)
     try:
@@ -162,8 +174,25 @@ def test_banded_host_call_matches_single_band(case, bands):
     finally:
         ab.set_option(ab.OPT_HOST_BANDS, -1)
     assert cs.count_mismatch(one, many) == 0
-    if o.have_ref():
-        assert cs.count_mismatch(expected(case, src), many) == 0
+    key = cs.case_id(case)
+    if key not in _banded_expected:
+        _banded_expected[key] = expected(case, src)
+    assert cs.count_mismatch(_banded_expected[key], many) == 0
+
+
+@pytest.mark.parametrize("bands", [2, 3, 7, 16])
+@pytest.mark.parametrize("case", BANDED, ids=cs.case_id)
+def test_banded_host_call_matches_single_band(case, bands):
+    """avirb200_resize_host cuts large images into row bands so that PCIe transfers overlap the
+    kernels; the band count must not change a bit (the HOST_BANDS plan option forces it)."""
+    _check_banded(case, bands)
+
+
+@pytest.mark.parametrize("bands", [2, 3, 7, 16])
+@pytest.mark.parametrize("case", BANDED, ids=cs.case_id)
+def test_banded_host_call_matches_single_band_per_family(case, bands, other_family):
+    """The same with the passes forced onto the tile kernel / the generic kernel (KERNEL_FAMILY)."""
+    _check_banded(case, bands)
 
 
 def test_banded_host_call_in_place():
@@ -320,11 +349,13 @@ def test_full_size_properties_cfg4():
     assert cs.count_mismatch(whole, d_dst.cpu().numpy()) == 0
 
 
-@needs_ref
-@pytest.mark.parametrize("nranks", [2, 5, 8])
-def test_sharded_local_matches_unsharded(nranks):
+SHARDED_LOCAL = [(2, 640, 720, 320, 360, 4, np.float32, np.float32, 16, {}),
+                 (0, 512, 600, 256, 300, 3, np.uint8, np.uint8, 8, {}),         # widened RGB
+                 (1, 640, 720, 320, 360, 1, np.float32, np.float32, 16, {})]    # widened gray
+
+
+def _check_sharded_local(case, nranks, family):
     import torch
-    case = (2, 640, 720, 320, 360, 4, np.float32, np.float32, 16, {})
     fp, sw, sh, nw, nh, ch, ti, to, rb, kw = case
     src = cs.make_input(case, seed=21)
     ref = cs.ref_output(case, src)
@@ -333,22 +364,40 @@ def test_sharded_local_matches_unsharded(nranks):
     lib = ab.lib()
     plan = C.c_void_p()
     assert lib.avirb200_plan_create(C.c_void_p(dp), C.byref(plan)) == 0
+    lib.avirb200_plan_set_option.argtypes = [C.c_void_p, C.c_int, C.c_int]
+    assert lib.avirb200_plan_set_option(plan, ab.OPT_KERNEL_FAMILY, family) == 0
     total = 0
     for r in range(nranks):
         b = C.c_size_t()
         assert lib.avirb200_shard_workspace_bytes(plan, r, nranks, C.byref(b)) == 0
         total += b.value
     d_src = torch.from_numpy(src).cuda()
-    d_dst = torch.zeros((nh, nw, ch), dtype=torch.float32, device="cuda")
+    d_dst = torch.zeros(nh * nw * ch * np.dtype(to).itemsize, dtype=torch.uint8, device="cuda")
     d_ws = torch.empty(total, dtype=torch.uint8, device="cuda")
     lib.avirb200_resize_sharded_local.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t,
                                                   C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
     assert lib.avirb200_resize_sharded_local(plan, nranks, d_src.data_ptr(), sw * ch,
-                                             d_dst.data_ptr(), nw * ch, d_ws.data_ptr(), None) == 0
+                                             d_dst.data_ptr(), nw * ch, d_ws.data_ptr(), None) == 0, \
+        lib.avirb200_last_error()
     torch.cuda.synchronize()
     lib.avirb200_plan_destroy(plan)
     rs.free_descriptor(h)
-    assert cs.count_mismatch(ref, d_dst.cpu().numpy()) == 0
+    assert cs.count_mismatch(ref, d_dst.cpu().numpy().view(to).reshape(nh, nw, ch)) == 0
+
+
+@needs_ref
+@pytest.mark.parametrize("nranks", [2, 5, 8])
+def test_sharded_local_matches_unsharded(nranks):
+    _check_sharded_local(SHARDED_LOCAL[0], nranks, 0)
+
+
+@needs_ref
+@pytest.mark.parametrize("nranks", [2, 5, 8])
+@pytest.mark.parametrize("case,family", [(c, f) for c in SHARDED_LOCAL for f in (0, 2, 1) if (c, f) != (SHARDED_LOCAL[0], 0)],
+                         ids=lambda v: ("product", "generic", "tile")[v] if isinstance(v, int) else cs.case_id(v))
+def test_sharded_local_matches_unsharded_per_family(case, family, nranks):
+    """Widened 1- and 3-channel plans, and every kernel family (KERNEL_FAMILY), on the sharded schedule."""
+    _check_sharded_local(case, nranks, family)
 
 
 # The fused halo exchange (AVIRB200_OPT_OVERLAP_HALO = 3: the row kernel stores the neighbours' rows into
@@ -362,6 +411,7 @@ FUSED_LOCAL = [
     (2, 1024, 1536, 256, 384, 4, np.uint8, np.uint8, 8, {"gamma": True, "alpha": 3}),        # cfg5 chain, sRGB table
     (1, 640, 720, 320, 360, 4, np.uint8, np.uint8, 8, {}),                                   # integer source and output
     (0, 512, 600, 256, 300, 3, np.uint8, np.uint8, 8, {}),                                   # 3 channels on the 4-channel kernels
+    (1, 640, 720, 320, 360, 1, np.float32, np.float32, 16, {}),                              # 1 channel on the 4-channel kernels
 ]
 
 
@@ -369,6 +419,19 @@ FUSED_LOCAL = [
 @pytest.mark.parametrize("nranks", [2, 3, 5])
 @pytest.mark.parametrize("case", FUSED_LOCAL, ids=cs.case_id)
 def test_sharded_local_fused_exchange_matches_unsharded(case, nranks, overlap):
+    _check_fused_local(case, nranks, overlap, 0)
+
+
+@pytest.mark.parametrize("overlap", [3, 1])
+@pytest.mark.parametrize("nranks", [2, 3, 5])
+@pytest.mark.parametrize("case", FUSED_LOCAL, ids=cs.case_id)
+def test_sharded_local_fused_exchange_matches_unsharded_per_family(case, nranks, overlap, other_family):
+    """The same with the passes forced onto the tile kernel / the generic kernel (KERNEL_FAMILY): the
+    exchange then takes the copied-halo schedule, on the same intermediate layout."""
+    _check_fused_local(case, nranks, overlap, other_family)
+
+
+def _check_fused_local(case, nranks, overlap, family):
     import torch
     fp, sw, sh, nw, nh, ch, ti, to, rb, kw = case
     src = cs.make_input(case, seed=33)
@@ -381,6 +444,7 @@ def test_sharded_local_fused_exchange_matches_unsharded(case, nranks, overlap):
     try:
         lib.avirb200_plan_set_option.argtypes = [C.c_void_p, C.c_int, C.c_int]
         assert lib.avirb200_plan_set_option(plan, ab.OPT_OVERLAP_HALO, overlap) == 0
+        assert lib.avirb200_plan_set_option(plan, ab.OPT_KERNEL_FAMILY, family) == 0
         total = 0
         for r in range(nranks):
             b = C.c_size_t()

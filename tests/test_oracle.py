@@ -289,3 +289,47 @@ def test_lancir_port_fuzz_matches_upstream():
                                             dst.ctypes.data, nw * ch) == 0
         h.lancirb200_host_desc_free(hd)
         assert cs.count_mismatch(ref, dst) == 0, (sw, sh, nw, nh, ch, ti, to, kw)
+
+
+# ---- upstream on padded buffers: the reference of the GPU layout tests (tests/test_gpu_layouts.py) ----
+
+@needs_ref
+@pytest.mark.parametrize("offset", [0, 1])
+@pytest.mark.parametrize("case", [
+    (2, 192, 108, 96, 54, 4, np.float32, np.float32, 16, {}),
+    (1, 256, 256, 64, 64, 4, np.uint16, np.uint16, 16, {}),
+    (2, 384, 216, 96, 54, 4, np.uint8, np.uint8, 8, {"gamma": True, "alpha": 3}),
+    (0, 320, 240, 160, 120, 3, np.uint8, np.uint8, 8, {}),
+    (1, 192, 108, 96, 54, 1, np.float32, np.float32, 16, {}),
+    (1, 192, 108, 96, 54, 4, np.float64, np.float64, 16, {}),
+    (4, 120, 80, 60, 40, 4, np.uint8, np.uint8, 8, {}),
+], ids=cs.case_id)
+def test_upstream_avir_ignores_source_padding(case, offset):
+    """Upstream with SrcScanlineSize on a source whose padding is NaN / the type's maximum gives the
+    bits of the packed copy."""
+    fp, sw, sh, nw, nh, ch, ti, to, rb, kw = case
+    src = cs.make_input(case, seed=12)
+    sl = cs.source_layout(src, 7, offset)
+    padded = o.ref_resize(sl.view(), nw, nh, to, fpclass=fp, resbits=rb, src_pitch=sl.pitch, **cs.ref_kwargs(kw))
+    assert cs.count_mismatch(cs.ref_output(case, src), padded) == 0
+
+
+@needs_ref
+@pytest.mark.parametrize("c", [
+    (96, 54, 48, 27, np.uint8, np.uint8, 4),
+    (64, 48, 103, 77, np.uint16, np.float32, 4),
+    (50, 30, 33, 17, np.float32, np.uint8, 3),
+    (96, 54, 48, 27, np.float32, np.float32, 1),
+])
+def test_upstream_lancir_scanline_sizes(c):
+    """Upstream CLancIR with SrcSSize / NewSSize: the packed bits, and not a byte of the destination's
+    padding or guard rows touched."""
+    sw, sh, nw, nh, ti, to, ch = c
+    src = o.lcg_image(sh, sw, ch, ti, seed=13)
+    sl = cs.source_layout(src, 5, 1)
+    dl = cs.guarded_dest((nh, nw, ch), to, 3, 1)
+    r, _ = o.lancir_ref(sl.view(), nw, nh, to, srcssize=sl.pitch, newssize=dl.pitch, dst=dl.view())
+    assert r == nh
+    r, want = o.lancir_ref(src, nw, nh, to)
+    assert cs.count_mismatch(want, np.ascontiguousarray(dl.view())) == 0
+    assert cs.guard_damage(dl) == 0

@@ -308,3 +308,40 @@ def test_stream_kernel_emulation_fuzz(emul):
         assert cs.count_mismatch(want, got) == 0, (cs.case_id(case), wh, wv, bands, var)
         ran += 1
     assert ran >= 30
+
+
+# Caller layouts: the source rows padded (pitch % 4 == 0 keeps the pass on the streaming kernel) with
+# poison in the padding, the destination rows padded and every byte outside the image a sentinel.
+@pytest.mark.parametrize("fused", [False, True], ids=["copied-halo", "fused"])
+@pytest.mark.parametrize("ec", EMUL_CASES[::5], ids=_id)
+def test_stream_kernel_emulation_padded_pitches(emul, ec, fused):
+    case, wh, wv, bands = ec
+    fp, sw, sh, nw, nh, ch, ti, to, rb, kw = case
+    if fused:
+        bands = max(bands, 2)
+    src = cs.make_input(case)
+    sl = cs.source_layout(src, 12)
+    dl = cs.guarded_dest((nh, nw, ch), to, 10)
+    rs, v = cs.resizer_and_vars(case)
+    h, dp, modes = rs.descriptor(src.shape, src.dtype, nw, nh, to, kw.get("k", 0.0), v)
+    try:
+        lut = np.zeros(256, np.float32)
+        cs.port().avir_port_srgb_lut(lut.ctypes.data)
+        s_ptr, d_ptr = sl.view().ctypes.data, dl.view().ctypes.data
+        if fused:
+            infos = band_infos(dp, bands)
+            if infos is None:
+                pytest.skip("bands too small for the sharded schedule")
+            rc = emul.stream_emul_resize_fused(dp, s_ptr, sl.pitch, d_ptr, dl.pitch, wh, wv, bands, 0,
+                                               lut.ctypes.data, 1, infos)
+            if rc == 1:
+                pytest.skip("a strip with rows of both neighbours: the product pushes with the copy engines")
+            assert rc == 0
+        else:
+            assert emul.stream_emul_resize(dp, s_ptr, sl.pitch, d_ptr, dl.pitch, wh, wv, bands, 1,
+                                           lut.ctypes.data, 1, band_needs(dp, bands), wh % 7, wv % 5) == 0
+    finally:
+        rs.free_descriptor(h)
+    want, _ = cs.port_output(case, src)
+    assert cs.count_mismatch(want, np.ascontiguousarray(dl.view())) == 0
+    assert cs.guard_damage(dl) == 0

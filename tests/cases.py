@@ -112,6 +112,127 @@ def make_input(case, seed=7, structured=None):
     return img
 
 
+# ---- the value domain: samples outside [0, 1], non-finite, subnormal, on rounding ties ---------------
+
+PATCH = 48  # constant patches: big enough that the filter output inside equals the patch value
+F32_MAX = float(np.finfo(np.float32).max)
+# patch values of the "huge" kind: far outside the output range, and either side of 2^31 once
+# multiplied by OutMul = 255 (u8 output) and 65535 (u16 output) -- where (int) leaves int32
+HUGE_VALUES = [1e6, -1e6, 1e8, -1e8, 1e30, -1e30]
+for _m in (255.0, 65535.0):
+    _b = np.float32(2.0 ** 31 / _m)
+    for _v in (np.nextafter(_b, np.float32(0)), np.nextafter(_b, np.float32(np.inf))):
+        HUGE_VALUES += [float(_v), -float(_v)]
+NONFINITE_VALUES = [np.inf, -np.inf, -np.nan, 3e38, F32_MAX, -F32_MAX]
+VALUE_KINDS = ("range", "huge", "nonfinite", "tiny", "ties")   # float sources
+INT_KINDS = ("every_code", "zero", "max")                       # integer sources
+
+
+def _patches(img, values, rng, size=PATCH):
+    """size x size patches on a grid, at least `size` apart (a filter's reach at k <= 4: 1e30 in one
+    patch must not swamp its neighbour), each channel of a patch constant at the next of `values`;
+    (y, x, channel, value) of every patch centre."""
+    sh, sw, ch = img.shape
+    size = min(size, sh, sw)
+    ny, nx = max(sh // (2 * size), 1), max(sw // (2 * size), 1)
+    gy, gx = (sh - ny * size) // (ny + 1), (sw - nx * size) // (nx + 1)
+    off = int(rng.integers(0, len(values)))
+    centres = []
+    for i in range(ny * nx):
+        y0, x0 = gy + (i // nx) * (size + gy), gx + (i % nx) * (size + gx)
+        for c in range(ch):
+            v = values[(off + i * ch + c) % len(values)]
+            img[y0:y0 + size, x0:x0 + size, c] = v
+            centres.append((y0 + size // 2, x0 + size // 2, c, v))
+    return centres
+
+
+def _sparse(img, values, rng, count):
+    """`count` single samples of `values` in turn at random positions and channels."""
+    sh, sw, ch = img.shape
+    for i in range(count):
+        img[int(rng.integers(0, sh)), int(rng.integers(0, sw)), int(rng.integers(0, ch))] = values[i % len(values)]
+
+
+def value_image(case, kind, seed=11):
+    """A seeded source image of `kind` for the case's geometry and input type.
+
+    Float sources (float32, or float64 with values beyond float32's range where noted):
+      range      uniform in [-4, 4]: both sides of the output clamp, the sRGB polynomial outside [0, 1]
+      huge       PATCH x PATCH constant patches of HUGE_VALUES on a [0, 1) background
+      nonfinite  sparse +-Inf, a negative quiet NaN, 3e38 (where lin2srgb_batch_ok stops) and
+                 +-FLT_MAX on a [0, 1) background
+      tiny       subnormals of both signs down to 2^-149, +-0.0 and a few +-FLT_MIN
+      ties       constant patches at (2k + 1) / (2 OutMul) and their float neighbours: outputs on
+                 k + 0.5, where the rounding modes differ
+    float64 sources add 1e39 / 1e300 (Inf once cast to float) and double subnormals.
+    Integer sources:
+      every_code every code of the type in every channel (u8: each channel 64 times over)
+      zero, max  all-zero and all-maximum images."""
+    fp, sw, sh, nw, nh, ch, ti, to, rb, kw = case
+    ti = np.dtype(ti)
+    rng = np.random.default_rng(seed)
+    if ti.kind != "f":
+        mx = np.iinfo(ti).max
+        if kind == "zero":
+            return np.zeros((sh, sw, ch), ti)
+        if kind == "max":
+            return np.full((sh, sw, ch), mx, ti)
+        assert kind == "every_code"
+        n = sh * sw
+        assert n >= mx + 1, "image too small for every code"
+        img = np.empty((sh, sw, ch), ti)
+        for c in range(ch):
+            img[..., c] = rng.permutation(np.arange(n) % (mx + 1)).astype(ti).reshape(sh, sw)
+        return img
+    img = rng.random((sh, sw, ch))
+    if kind == "range":
+        img = rng.uniform(-4.0, 4.0, (sh, sw, ch))
+    elif kind == "huge":
+        _patches(img, HUGE_VALUES, rng)
+    elif kind == "nonfinite":
+        _sparse(img, NONFINITE_VALUES, rng, max(6, sh * sw // 1500))
+    elif kind == "tiny":
+        sub = rng.integers(0, 1 << 23, (sh, sw, ch)).astype(np.float64) * 2.0 ** -149
+        sub[rng.random((sh, sw, ch)) < 0.1] = 0.0
+        sub[rng.random((sh, sw, ch)) < 0.02] = 2.0 ** -126
+        sub.ravel()[:8] = 2.0 ** -149
+        img = np.where(rng.random((sh, sw, ch)) < 0.5, -sub, sub)
+    elif kind == "ties":
+        mul = {np.dtype(u8): 255.0, np.dtype(u16): 65535.0}.get(np.dtype(to), 255.0)
+        levels = []
+        for k_ in rng.integers(0, int(mul), 6):
+            t = np.float32((2 * int(k_) + 1) / (2 * mul))
+            levels += [float(np.nextafter(t, np.float32(-1))), float(t), float(np.nextafter(t, np.float32(2)))]
+        _patches(img, levels, rng)
+    else:
+        raise ValueError(kind)
+    if ti == np.float64:
+        _sparse(img, [1e39, -1e39, 1e300, -1e300, 5e-324, -5e-324, 1e-310], rng, max(7, sh * sw // 1500))
+        return img
+    return img.astype(np.float32)
+
+
+def huge_patch_centres(case, seed=11):
+    """(y, x, channel, value) of the centres of value_image(case, "huge", seed)'s patches."""
+    fp, sw, sh, nw, nh, ch, ti, to, rb, kw = case
+    rng = np.random.default_rng(seed)
+    img = rng.random((sh, sw, ch))
+    return _patches(img, HUGE_VALUES, rng)
+
+
+def value_mismatch(want, got):
+    """Elements that differ: integers exactly; floats bit for bit except that any NaN matches any
+    NaN (payloads are not preserved, positions are), so +-0 and +-Inf count."""
+    assert want.shape == got.shape and want.dtype == got.dtype
+    if want.dtype.kind != "f":
+        return int((want != got).sum())
+    nw_, ng = np.isnan(want), np.isnan(got)
+    bits = np.uint32 if want.dtype == np.float32 else np.uint64
+    differ = (want.view(bits) != got.view(bits)) & ~(nw_ & ng)
+    return int(differ.sum())
+
+
 def ref_kwargs(kw):
     return dict(k=kw.get("k", 0.0), ox=kw.get("ox", 0.0), oy=kw.get("oy", 0.0),
                 gamma=kw.get("gamma", False), alpha=kw.get("alpha", -1),

@@ -5,6 +5,9 @@ Run in the build container (where /root/reference exists):
     python tests/golden/make_golden.py
 Each avir_*.npz holds: case tuple, seeded input image, upstream's output image.
 Each lancir_*.npz holds: geometry, input, upstream CLancIR output.
+Each value_*.npz holds: case tuple, value kind (cases.value_image), input, upstream's output -- the
+value domain (huge, non-finite, subnormal samples), whose float outputs carry NaN: they are compared
+NaN-aware (cases.value_mismatch), not bit for bit like avir_*.
 Fixtures are small (<= ~100 KB each) so they can live in git.
 """
 import os
@@ -42,6 +45,17 @@ GOLDEN_CASES = [
     (0, 60, 40, 45, 50, 3, f64, u16, 16, {"gamma": True}),
 ]
 
+# (case, cases.value_image kind): default class (round() beyond int32) and float8_dil class
+VALUE_FIXTURES = [
+    ((0, 96, 64, 48, 32, 4, f32, u8, 8, {"buildmode": 1}), "huge"),
+    ((0, 96, 64, 48, 32, 4, f32, u8, 8, {"buildmode": 1}), "nonfinite"),
+    ((0, 64, 48, 32, 24, 4, f32, f32, 16, {}), "tiny"),
+    ((2, 96, 64, 48, 32, 4, f32, f32, 16, {"buildmode": 1}), "nonfinite"),
+    ((2, 96, 64, 48, 32, 4, f32, u8, 8, {"buildmode": 1}), "huge"),
+    ((2, 64, 48, 32, 24, 4, f32, f32, 16, {"buildmode": 1}), "tiny"),
+    ((3, 96, 64, 48, 32, 4, f32, u8, 8, {}), "huge"),
+]
+
 LANCIR_CASES = [
     (96, 54, 48, 27, u8, u8, {}),
     (64, 48, 103, 77, u8, u8, {}),
@@ -71,6 +85,14 @@ def main():
         c[7] = np.dtype(c[7]).name
         np.savez_compressed(os.path.join(HERE, "avir_%02d.npz" % i),
                             case=np.array(c, dtype=object), src=src, out=out)
+    for i, (case, kind) in enumerate(VALUE_FIXTURES):
+        src = cs.value_image(case, kind)
+        out = cs.ref_output(case, src)
+        c = list(case)
+        c[6] = np.dtype(c[6]).name
+        c[7] = np.dtype(c[7]).name
+        np.savez_compressed(os.path.join(HERE, "value_%02d.npz" % i),
+                            case=np.array(c, dtype=object), kind=kind, src=src, out=out)
     for i, (sw, sh, nw, nh, ti, to, kw) in enumerate(LANCIR_CASES):
         src = o.lcg_image(sh, sw, 4, ti, seed=200 + i)
         r, out = o.lancir_ref(src, nw, nh, to, **kw)
@@ -83,7 +105,7 @@ def main():
         assert r == nh
         np.savez_compressed(os.path.join(HERE, "lancir_%02d.npz" % (len(LANCIR_CASES) + i)),
                             src=src, out=out, geom=np.array([sw, sh, nw, nh]))
-    print("wrote", len(GOLDEN_CASES), "AVIR and", len(LANCIR_CASES), "LANCIR fixtures;",
+    print("wrote", len(GOLDEN_CASES), "AVIR,", len(VALUE_FIXTURES), "value-domain and", len(LANCIR_CASES), "LANCIR fixtures;",
           o.ref().avir_ref_version().decode())
 
 

@@ -15,6 +15,7 @@ import oracle_ref as o
 import plan_util as pu
 
 needs_ref = pytest.mark.skipif(not o.have_ref(), reason="oracle/_ref not built")
+u8, u16, f32, f64 = np.uint8, np.uint16, np.float32, np.float64
 
 
 def hexf(strs):
@@ -112,6 +113,69 @@ def test_port_structured_inputs(case, structured):
     src = cs.make_input(case, structured=structured)
     mine, _ = cs.port_output(case, src)
     assert cs.count_mismatch(cs.ref_output(case, src), mine) == 0
+
+
+# the port stays a valid oracle outside [0, 1]: out-of-int32 rounding, non-finite and subnormal samples
+# (floats compared NaN-aware: upstream passes NaN payloads through, the port's arithmetic may not)
+VALUE_CASES = [
+    (0, 256, 192, 128, 96, 4, f32, u8, 8, {"buildmode": 1}),
+    (0, 256, 192, 64, 48, 4, f32, u16, 16, {}),
+    (0, 200, 150, 100, 75, 3, f32, u8, 8, {"gamma": True}),
+    (1, 256, 192, 128, 96, 4, f32, u8, 8, {}),
+    (2, 256, 192, 64, 48, 4, f32, u16, 16, {"buildmode": 1}),
+    (2, 256, 192, 128, 96, 4, f32, f32, 16, {"gamma": True}),
+    (0, 150, 90, 100, 55, 4, f32, u16, 12, {}),
+    (3, 256, 192, 128, 96, 4, f32, u8, 8, {}),
+    (4, 256, 192, 128, 96, 4, f32, u16, 16, {}),
+    (5, 256, 192, 128, 96, 4, f32, u8, 6, {"gamma": True, "alpha": 3}),
+    (5, 256, 192, 64, 48, 4, f32, u16, 16, {"buildmode": 1}),
+    (0, 120, 80, 60, 40, 3, f32, f64, 16, {"gamma": True}),
+    (1, 192, 108, 96, 54, 4, f64, u16, 16, {}),
+]
+
+
+@needs_ref
+@pytest.mark.parametrize("kind", cs.VALUE_KINDS)
+@pytest.mark.parametrize("case", VALUE_CASES, ids=cs.case_id)
+def test_port_value_domain_matches_upstream(case, kind):
+    src = cs.value_image(case, kind)
+    mine, _ = cs.port_output(case, src)
+    assert cs.value_mismatch(cs.ref_output(case, src), mine) == 0
+
+
+@needs_ref
+@pytest.mark.parametrize("case", [c for c in VALUE_CASES if c[0] in (0, 3) and c[7] in (u8, u16)
+                                  and not c[9].get("gamma") and c[8] in (8, 16)], ids=cs.case_id)
+def test_upstream_wraps_beyond_int32(case):
+    """Upstream's round() is -(int)(0.5 - v) / (int)(v + 0.5) on x86, where (int) yields INT_MIN
+    outside int32: a patch scaled (by OutMul) beyond +2^31 gives 0 and one beyond -2^31 gives PkOut
+    -- the "huge" kind does reach that quirk.  (Near 1e30 * OutMul upstream's own filter arithmetic
+    overflows in places, so the negative side is checked at +-1e8 and +-1e6.)"""
+    fp, sw, sh, nw, nh, ch, ti, to, rb, kw = case
+    out = cs.ref_output(case, cs.value_image(case, "huge"))
+    pk, mul = np.iinfo(to).max, float(np.iinfo(to).max)
+    seen = set()
+    for y, x, c, v in cs.huge_patch_centres(case):
+        got = out[y * nh // sh, x * nw // sw, c]
+        if v * mul > 1.01 * 2.0 ** 31:
+            assert got == 0, (v, y, x, c)
+            seen.add("wrap to 0")
+        elif -1e20 < v * mul < -1.01 * 2.0 ** 31:
+            assert got == pk, (v, y, x, c)
+            seen.add("wrap to PkOut")
+    assert seen == {"wrap to 0", "wrap to PkOut"}
+
+
+def test_port_matches_value_fixtures():
+    files = sorted(f for f in os.listdir(cs.GOLDEN) if f.startswith("value_") and f.endswith(".npz"))
+    assert len(files) >= 6
+    for f in files:
+        z = np.load(os.path.join(cs.GOLDEN, f), allow_pickle=True)
+        case = tuple(z["case"].tolist())
+        case = case[:6] + (np.dtype(case[6]).type, np.dtype(case[7]).type) + case[8:]
+        assert z["src"].tobytes() == cs.value_image(case, str(z["kind"])).tobytes(), f
+        mine, _ = cs.port_output(case, z["src"])
+        assert cs.value_mismatch(z["out"], mine) == 0, f
 
 
 def test_port_matches_golden_fixtures():

@@ -310,6 +310,46 @@ def test_stream_kernel_emulation_fuzz(emul):
     assert ran >= 30
 
 
+# The value domain (cases.value_image): samples outside [0, 1], beyond int32 once scaled to the
+# output range, non-finite and subnormal, through the output stage of every chain.  The emulation's
+# float-to-int conversions model the device's (NaN to 0, saturating), so this is where a difference
+# from upstream's x86 conversions shows up without a GPU.
+VALUE_EMUL_CASES = [
+    ((0, 100, 70, 50, 35, 4, f32, u8, 8, {"buildmode": 1}), 4, 3, 2),      # default class, k = 2
+    ((0, 256, 192, 128, 96, 4, f32, u8, 8, {"buildmode": 1}), 3, 2, 1),    # every huge patch
+    ((0, 256, 192, 128, 96, 4, f32, u16, 16, {"buildmode": 1}), 2, 5, 3),
+    ((0, 128, 96, 256, 192, 4, f32, u16, 16, {"buildmode": 1}), 3, 2, 1),  # cfg2 chain
+    ((0, 256, 192, 64, 48, 4, f32, u8, 8, {"buildmode": 0}), 2, 2, 2),     # cfg4 chain
+    ((1, 256, 192, 128, 96, 4, f32, u8, 8, {"buildmode": 1}), 4, 3, 2),    # RNE_I32
+    ((1, 256, 192, 64, 48, 4, f32, u16, 16, {"buildmode": 0}), 3, 2, 1),
+    ((2, 256, 192, 128, 96, 4, f32, u16, 16, {"buildmode": 1}), 2, 2, 1),  # RNE
+    ((2, 256, 192, 64, 48, 4, f32, u8, 8, {"buildmode": 1}), 3, 4, 2),     # cfg5 chain
+    ((2, 256, 192, 128, 96, 4, f32, f32, 16, {"buildmode": 1}), 3, 2, 1),  # float output
+    ((1, 256, 192, 128, 96, 4, f32, f32, 16, {"buildmode": 0}), 2, 3, 2),
+]
+
+
+@pytest.mark.parametrize("kind", ("range", "huge", "nonfinite", "tiny"))
+@pytest.mark.parametrize("ec", VALUE_EMUL_CASES, ids=_id)
+def test_stream_kernel_emulation_value_domain(emul, ec, kind):
+    case, wh, wv, bands = ec
+    fp, sw, sh, nw, nh, ch, ti, to, rb, kw = case
+    src = cs.value_image(case, kind)
+    rs, v = cs.resizer_and_vars(case)
+    h, dp, modes = rs.descriptor(src.shape, src.dtype, nw, nh, to, kw.get("k", 0.0), v)
+    try:
+        assert emul.stream_emul_applicable(dp) == 1, "chain not on the streaming kernel: %r" % (modes,)
+        got = np.zeros((nh, nw, ch), to)
+        lut = np.zeros(256, np.float32)
+        cs.port().avir_port_srgb_lut(lut.ctypes.data)
+        assert emul.stream_emul_resize(dp, src.ctypes.data, sw * ch, got.ctypes.data, nw * ch, wh, wv, bands,
+                                       1, lut.ctypes.data, 1, band_needs(dp, bands), wh % 7, wv % 5) == 0
+    finally:
+        rs.free_descriptor(h)
+    want, _ = cs.port_output(case, src)
+    assert cs.value_mismatch(want, got) == 0
+
+
 # Caller layouts: the source rows padded (pitch % 4 == 0 keeps the pass on the streaming kernel) with
 # poison in the padding, the destination rows padded and every byte outside the image a sentinel.
 @pytest.mark.parametrize("fused", [False, True], ids=["copied-halo", "fused"])

@@ -29,33 +29,22 @@
 #include "device_plan.h"
 #include "fast_pass.cuh"
 #include "generic_pass.cuh"
+#include "host_util.h"
 #include "stream_types.h"
 #include "stream_launch.h"
 
 using namespace avb;
 
 namespace {
-
 thread_local std::string g_err;
+}
 
-int fail(int code, const std::string& msg) {
+int avb::fail(int code, const std::string& msg) {
     g_err = msg;
     return code;
 }
 
-#define CUDA_TRY(expr)                                                                       \
-    do {                                                                                     \
-        cudaError_t e_ = (expr);                                                             \
-        if (e_ != cudaSuccess)                                                               \
-            return fail(e_ == cudaErrorMemoryAllocation ? AVIRB200_ERR_ALLOC                 \
-                                                        : (e_ == cudaErrorNoDevice ||        \
-                                                           e_ == cudaErrorInsufficientDriver \
-                                                               ? AVIRB200_ERR_NO_DEVICE      \
-                                                               : AVIRB200_ERR_CUDA),         \
-                        std::string(#expr) + ": " + cudaGetErrorString(e_));                 \
-    } while (0)
-
-size_t dtype_size(int t) { return t == AVIRB200_U8 ? 1 : (t == AVIRB200_U16 ? 2 : (t == AVIRB200_F64 ? 8 : 4)); }
+namespace {
 
 // The u8 sRGB->linear table: upstream ships 256 float literals (avir.h:234-286) that equal
 // the double-precision linearisation formula printed with 7 significant digits.  Regenerated
@@ -152,7 +141,6 @@ int copy_axis_host(HostAxis& ha, const avirb200_axis_desc& ad) {
     ha.taps.resize(n); ha.frac.resize(n); ha.pdc.resize(n); ha.sdc.resize(n);
     ha.src_pos.resize(n); ha.phase.resize(n);
     int prev_len = ad.src_len;
-    int prev_lo = 0, prev_hi = ad.src_len;
     for (int i = 0; i < n; ++i) {
         const avirb200_step_desc& s = ad.steps[i];
         if (s.in_len != prev_len && !(s.kind == AVIRB200_STEP_RESIZE && s.upsampled))
@@ -186,14 +174,18 @@ int copy_axis_host(HostAxis& ha, const avirb200_axis_desc& ad) {
             }
         }
         ha.taps[i].assign(s.taps, s.taps + nt);
-        (void)prev_lo; (void)prev_hi;
         prev_len = s.out_len;
     }
     if (prev_len != ad.dst_len) return fail(AVIRB200_ERR_BAD_ARG, "axis: chain does not end at dst_len");
+    // from here on the descriptor points at the plan's own copies of the tables
+    for (int i = 0; i < n; ++i) {
+        avirb200_step_desc& sd = ha.desc.steps[i];
+        sd.taps = ha.taps[i].data(); sd.src_pos = ha.src_pos[i].data();
+        sd.phase = ha.phase[i].data(); sd.frac = ha.frac[i].data();
+        sd.prefix_dc = ha.pdc[i].data(); sd.suffix_dc = ha.sdc[i].data();
+    }
     return 0;
 }
-
-size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 size_t axis_arena_bytes(const HostAxis& ha) {
     size_t b = 0;
@@ -215,14 +207,15 @@ const T* stage(std::vector<char>& img, size_t& off, char* dbase, const std::vect
     return d;
 }
 
-void build_dev_axis(HostAxis& ha, std::vector<char>& img, size_t& off, char* dbase) {
-    DevAxis& d = ha.dev;
-    d.src_len = ha.desc.src_len;
-    d.dst_len = ha.desc.dst_len;
-    d.nsteps = ha.desc.nsteps;
-    int lo = 0, hi = ha.desc.src_len;
-    for (int i = 0; i < d.nsteps; ++i) {
-        const avirb200_step_desc& s = ha.desc.steps[i];
+// The kernels' view of an axis descriptor, with the descriptor's (host) table pointers: what the
+// range arithmetic reads.
+DevAxis host_axis_view(const avirb200_axis_desc& ad) {
+    DevAxis d;
+    std::memset(&d, 0, sizeof d);
+    d.src_len = ad.src_len; d.dst_len = ad.dst_len; d.nsteps = ad.nsteps;
+    int lo = 0, hi = ad.src_len;
+    for (int i = 0; i < ad.nsteps && i < AVIRB200_MAX_STEPS; ++i) {
+        const avirb200_step_desc& s = ad.steps[i];
         DevStep& ds = d.steps[i];
         ds.kind = s.kind; ds.resample = s.resample; ds.latency = s.latency; ds.edge = s.edge;
         ds.in_len = s.in_len; ds.out_len = s.out_len; ds.ntaps = s.ntaps; ds.order = s.order;
@@ -232,22 +225,26 @@ void build_dev_axis(HostAxis& ha, std::vector<char>& img, size_t& off, char* dba
         ds.in_prefix = s.in_prefix; ds.in_suffix = s.in_suffix;
         ds.n_prefix_dc = s.n_prefix_dc; ds.n_suffix_dc = s.n_suffix_dc;
         ds.in_lo = lo; ds.in_hi = hi;
+        ds.taps = s.taps; ds.src_pos = s.src_pos; ds.phase = s.phase; ds.frac = s.frac;
+        ds.prefix_dc = s.prefix_dc; ds.suffix_dc = s.suffix_dc;
+        const Range od = step_output_domain(ds);
+        lo = od.a; hi = od.b + 1;
+    }
+    return d;
+}
+
+// hostdev: the axis with the plan's host copies of the tables; dev: the same with the copies staged
+// into the plan's device arena.
+void build_dev_axis(HostAxis& ha, std::vector<char>& img, size_t& off, char* dbase) {
+    ha.hostdev = ha.dev = host_axis_view(ha.desc);
+    for (int i = 0; i < ha.dev.nsteps; ++i) {
+        DevStep& ds = ha.dev.steps[i];
         ds.taps = stage(img, off, dbase, ha.taps[i]);
         ds.src_pos = stage(img, off, dbase, ha.src_pos[i]);
         ds.phase = stage(img, off, dbase, ha.phase[i]);
         ds.frac = stage(img, off, dbase, ha.frac[i]);
         ds.prefix_dc = stage(img, off, dbase, ha.pdc[i]);
         ds.suffix_dc = stage(img, off, dbase, ha.sdc[i]);
-        const Range od = step_output_domain(ds);
-        lo = od.a;
-        hi = od.b + 1;
-    }
-    ha.hostdev = d;
-    for (int i = 0; i < d.nsteps; ++i) {
-        ha.hostdev.steps[i].src_pos = ha.src_pos[i].empty() ? nullptr : ha.src_pos[i].data();
-        ha.hostdev.steps[i].taps = ha.taps[i].data();
-        ha.hostdev.steps[i].phase = ha.phase[i].empty() ? nullptr : ha.phase[i].data();
-        ha.hostdev.steps[i].frac = ha.frac[i].empty() ? nullptr : ha.frac[i].data();
     }
 }
 
@@ -328,29 +325,33 @@ int launch_narrow(int type, const void* src, void* dst, size_t dst_pitch, int w,
 
 // 1..3-channel plans whose passes run on the 4-channel kernels in this call (avirb200_plan::pad4)
 bool use_pad4(const avirb200_plan* pl) { return pl->pad4 && pl->opt_family != 1; }
-bool row_pass_can_segment(const avirb200_plan* pl, const void* d_src, size_t src_pitch, const float* d_mid) {
-    return pl->opt_family == 0 && pl->stream_h.chain != 0 && !use_pad4(pl) &&
-           ((uintptr_t)d_src % (4 * dtype_size(pl->desc.in_type))) == 0 && (src_pitch % 4) == 0 && ((uintptr_t)d_mid % 16) == 0;
+
+// Floats between consecutive intermediate rows, for every kernel family and every band / halo offset.
+size_t mid_pitch(const avirb200_plan* pl) { return (size_t)pl->desc.dst_w * pl->mid_ch; }
+
+// Whether a pass runs on the streaming kernel with these buffers (the kernel's source / destination as
+// it sees them: a widened plan's scratch copies).  The copies move whole pixels: the row pass's source
+// pixels and the column pass's channel pairs must be aligned to their size, the intermediate to 16 bytes.
+bool row_pass_on_stream(const avirb200_plan* pl, const void* src, size_t src_pitch, const float* mid) {
+    return pl->opt_family == 0 && pl->stream_h.chain != 0 && ((uintptr_t)src % (4 * elem_size(pl->desc.in_type))) == 0 &&
+           (src_pitch % 4) == 0 && ((uintptr_t)mid % 16) == 0;
 }
-size_t pad4_src_bytes(const avirb200_plan* pl, int rows) {
-    return pl->pad4 ? ((size_t)rows * pl->desc.src_w * 4 * dtype_size(pl->desc.in_type) + 255) / 256 * 256 : 0;
-}
-size_t pad4_dst_bytes(const avirb200_plan* pl, int rows) {
-    return pl->pad4 ? ((size_t)rows * pl->desc.dst_w * 4 * dtype_size(pl->desc.out_type) + 255) / 256 * 256 : 0;
+bool col_pass_on_stream(const avirb200_plan* pl, const void* dst, size_t dst_pitch, const float* mid) {
+    return pl->opt_family == 0 && pl->stream_v.chain != 0 && ((uintptr_t)dst % (2 * elem_size(pl->desc.out_type))) == 0 &&
+           (dst_pitch % 2) == 0 && ((uintptr_t)mid % 16) == 0;
 }
 
 // Row pass over `rows` source rows (band starting at d_src) into the intermediate band
 // starting at d_mid; column pass producing dst rows [out0, out1) from an intermediate
 // buffer whose row 0 is global row mid_row_base.
 // scratch4: where the band's widened (4-channel) copy goes when use_pad4(pl).
-// seg_top / seg_bot (streaming kernel, 4-channel plans only -- the caller checks row_pass_can_segment()):
-// filter only the band's first seg_top and last seg_bot rows, in ONE launch.
-bool row_pass_can_segment(const avirb200_plan* pl, const void* d_src, size_t src_pitch, const float* d_mid);
-// xs (sharded calls, fused halo exchange): the StreamParams xs_* fields of this launch; *xs_done tells
-// whether the streaming kernel took the pass (and so delivered the neighbours' rows).
+// seg_top / seg_bot (4-channel plans only, the caller checks row_pass_on_stream()): filter only the
+// band's first seg_top and last seg_bot rows, in ONE launch.
+// xs (sharded calls, fused halo exchange): the band's link, sent through the streaming kernel; *xs_done
+// tells whether the streaming kernel took the pass (and so delivered the neighbours' rows).
 int run_row_pass(const avirb200_plan* pl, const void* d_src, size_t src_pitch, float* d_mid,
                  int rows, cudaStream_t st, int* launches, void* scratch4 = nullptr, int seg_top = 0, int seg_bot = 0,
-                 const avs::StreamParams* xs = nullptr, bool* xs_done = nullptr) {
+                 const avs::StreamLink* xs = nullptr, bool* xs_done = nullptr) {
     if (rows <= 0) return 0;
     // (a non-sticky error another library left in this thread -- NCCL's peer-access probing leaves
     // cudaErrorPeerAccessAlreadyEnabled once the IPC mailboxes have enabled it -- is not this launch's)
@@ -365,47 +366,22 @@ int run_row_pass(const avirb200_plan* pl, const void* d_src, size_t src_pitch, f
         d_src = scratch4;
         src_pitch = (size_t)d.src_w * 4;
     }
-    if (pl->opt_family == 0 && pl->stream_h.chain != 0 &&
-        ((uintptr_t)d_src % (4 * dtype_size(d.in_type))) == 0 && (src_pitch % 4) == 0 &&
-        ((uintptr_t)d_mid % 16) == 0) {
-        // (every pixel of the source must be aligned to its own size: the copies move whole pixels)
+    if (row_pass_on_stream(pl, d_src, src_pitch, d_mid)) {
         avs::StreamParams sp;
-        avs::stream_fill_params(sp, pl->stream_h, d);
-        sp.src_type = avs::stream_row_source_code(d);
-        sp.srgb_lut = pl->d_lut;
-        sp.n_lines = rows;
-        if (seg_bot > 0) {
-            sp.seg_a = seg_top;
-            sp.seg_b = seg_bot;
-            sp.seg_b_line0 = rows - seg_bot;
-        } else if (seg_top > 0) {
-            sp.n_lines = seg_top;
-        }
-        sp.out0 = 0;
-        sp.out1 = d.dst_w;
-        sp.src = d_src;
-        sp.src_pitch = (long long)src_pitch;
-        sp.dst = d_mid;
-        sp.dst_pitch = (long long)d.dst_w * 4;
-        sp.dst_type = AVIRB200_F32;
-        if (xs != nullptr) {
-            sp.xs_up_dst = xs->xs_up_dst; sp.xs_dn_dst = xs->xs_dn_dst;
-            sp.xs_up_flag = xs->xs_up_flag; sp.xs_dn_flag = xs->xs_dn_flag;
-            sp.xs_count = xs->xs_count; sp.xs_units[0] = xs->xs_units[0]; sp.xs_units[1] = xs->xs_units[1];
-            sp.xs_seq = xs->xs_seq; sp.xs_top = xs->xs_top; sp.xs_bot0 = xs->xs_bot0; sp.xs_bot = xs->xs_bot;
-        }
+        avs::stream_fill_row_params(sp, pl->stream_h, d, d_src, (long long)src_pitch, d_mid, (long long)mid_pitch(pl), rows,
+                                    pl->d_lut, seg_top, seg_bot);
+        if (xs != nullptr) avs::stream_set_sender(sp, *xs);
         const int r = avs::stream_launch(pl->stream_h.chain, false, 0, pl->opt_var_h, sp, pl->sm_count, st);
         if (r == -1) return fail(AVIRB200_ERR_CUDA, "streaming row pass launch failed");
         if (r == 0) { ++*launches; if (xs_done) *xs_done = (xs != nullptr); return 0; }
     }
     if (pl->opt_family != 1 && pl->fast.h_ok) {
-        const int r = fast_row_pass(pl->fast, d, d_src, src_pitch, d_mid, rows, pl->d_lut, st);
+        const int r = fast_row_pass(pl->fast, d, d_src, src_pitch, d_mid, mid_pitch(pl), rows, pl->d_lut, pl->sm_count, st);
         if (r == -1) return fail(AVIRB200_ERR_CUDA, "fast row pass launch failed");
         if (r == 0) { ++*launches; return 0; }
     }
-    // The generic kernel.  Its intermediate rows are dst_w * mid_ch floats apart, as every other
-    // kernel family and every band / halo offset lays them out.  A widened band the 4-channel kernels
-    // did not take runs it on the widened copy with 4 channels (the pad channel's results are dropped).
+    // The generic kernel.  A widened band the 4-channel kernels did not take runs it on the widened
+    // copy with 4 channels (the pad channel's results are dropped).
     PassParams p;
     std::memset(&p, 0, sizeof p);
     fill_common(p, pl);
@@ -424,7 +400,7 @@ int run_row_pass(const avirb200_plan* pl, const void* d_src, size_t src_pitch, f
     p.src_pitch = (long long)src_pitch;
     p.src_type = d.in_type;
     p.dst = d_mid;
-    p.dst_pitch = (long long)d.dst_w * pl->mid_ch;
+    p.dst_pitch = (long long)mid_pitch(pl);
     p.dst_type = AVIRB200_F32;
     ++*launches;
     return launch_generic(p, c, st);
@@ -432,12 +408,12 @@ int run_row_pass(const avirb200_plan* pl, const void* d_src, size_t src_pitch, f
 
 // scratch4: where the band's 4-channel destination rows go when use_pad4(pl) (then narrowed into d_dst).
 // mid_rows: intermediate rows the buffer holds from mid_row_base on (< 0: up to the image's last row).
-// xr (sharded calls, fused halo exchange): the StreamParams xr_* fields -- the neighbours' rows are read in
-// place from the mailbox.  Returns 1, nothing launched, when the streaming kernel cannot take the pass
-// (the caller moves the rows into the workspace and calls again without xr).
+// xr (sharded calls, fused halo exchange): the band's link -- the neighbours' rows are read in place from
+// its mailbox.  Returns 1, nothing launched, when the streaming kernel cannot take the pass (the caller
+// moves the rows into the workspace and calls again without xr).
 int run_col_pass(const avirb200_plan* pl, const float* d_mid, int mid_row_base, void* d_dst,
                  size_t dst_pitch, int out0, int out1, cudaStream_t st, int* launches, void* scratch4 = nullptr,
-                 int mid_rows = -1, const avs::StreamParams* xr = nullptr) {
+                 int mid_rows = -1, const avs::StreamLink* xr = nullptr) {
     if (out1 <= out0) return 0;
     (void)cudaGetLastError(); // (see run_row_pass)
     const avirb200_plan_desc& d = pl->desc;
@@ -456,44 +432,27 @@ int run_col_pass(const avirb200_plan* pl, const float* d_mid, int mid_row_base, 
         ++*launches;
         return 0;
     };
-    {
-        const size_t es = fast_elsize(d.out_type);
-        if (pl->opt_family == 0 && pl->stream_v.chain != 0 &&
-            ((uintptr_t)d_dst % (2 * es)) == 0 && (dst_pitch % 2) == 0 && ((uintptr_t)d_mid % 16) == 0) {
-            avs::StreamParams sp;
-            avs::stream_fill_params(sp, pl->stream_v, d);
-            sp.n_lines = d.dst_w;
-            sp.out0 = out0;
-            sp.out1 = out1;
-            sp.src = d_mid;
-            sp.src_pitch = (long long)d.dst_w * 4;
-            sp.src_row_base = mid_row_base;
-            sp.src_lo = mid_row_base;
-            sp.src_hi = (mid_rows >= 0) ? mid_row_base + mid_rows : d.src_h;
-            sp.dst = d_dst;
-            sp.dst_pitch = (long long)dst_pitch;
-            sp.dst_type = d.out_type;
-            sp.dst_row_base = out0;
-            if (xr != nullptr) {
-                sp.xr_up_src = xr->xr_up_src; sp.xr_dn_src = xr->xr_dn_src; sp.xr_flags = xr->xr_flags;
-                sp.xr_seq = xr->xr_seq; sp.xr_own_lo = xr->xr_own_lo; sp.xr_own_hi = xr->xr_own_hi;
-            }
-            const int r = avs::stream_launch(pl->stream_v.chain, true, avs::stream_epilogue_code(d), pl->opt_var_v, sp,
-                                             pl->sm_count, st);
-            if (r == -1) return fail(AVIRB200_ERR_CUDA, "streaming column pass launch failed");
-            if (r == 0) { ++*launches; return finish(); }
-        }
-        if (xr != nullptr) return 1;
+    if (col_pass_on_stream(pl, d_dst, dst_pitch, d_mid)) {
+        avs::StreamParams sp;
+        avs::stream_fill_col_params(sp, pl->stream_v, d, d_mid, (long long)mid_pitch(pl), mid_row_base,
+                                    (mid_rows >= 0) ? mid_row_base + mid_rows : d.src_h, d_dst, (long long)dst_pitch,
+                                    out0, out1);
+        if (xr != nullptr) avs::stream_set_receiver(sp, *xr);
+        const int r = avs::stream_launch(pl->stream_v.chain, true, avs::stream_epilogue_code(d), pl->opt_var_v, sp,
+                                         pl->sm_count, st);
+        if (r == -1) return fail(AVIRB200_ERR_CUDA, "streaming column pass launch failed");
+        if (r == 0) { ++*launches; return finish(); }
     }
+    if (xr != nullptr) return 1;
     if (pl->opt_family != 1 && pl->fast.v_ok) {
-        const int r = fast_col_pass(pl->fast, d, d_mid, mid_row_base, d_dst, dst_pitch, out0, out1,
-                                    pl->d_lut, st);
+        const int r = fast_col_pass(pl->fast, d, d_mid, mid_pitch(pl), mid_row_base, d_dst, dst_pitch, out0, out1,
+                                    pl->d_lut, pl->sm_count, st);
         if (r == -1) return fail(AVIRB200_ERR_CUDA, "fast column pass launch failed");
         if (r == 0) { ++*launches; return finish(); }
     }
-    // The generic kernel (intermediate rows dst_w * mid_ch floats apart, see run_row_pass).  A widened
-    // band the tile kernel refused (a shard whose footprint exceeds its shared memory) runs it with 4
-    // channels into the 4-channel scratch, narrowed as after the 4-channel kernels.
+    // The generic kernel.  A widened band the tile kernel refused (a shard whose footprint exceeds its
+    // shared memory) runs it with 4 channels into the 4-channel scratch, narrowed as after the
+    // 4-channel kernels.
     PassParams p;
     std::memset(&p, 0, sizeof p);
     fill_common(p, pl);
@@ -510,7 +469,7 @@ int run_col_pass(const avirb200_plan* pl, const float* d_mid, int mid_row_base, 
     p.span = c.span;
     p.pitch = c.pitch;
     p.src = d_mid;
-    p.src_pitch = (long long)d.dst_w * pl->mid_ch;
+    p.src_pitch = (long long)mid_pitch(pl);
     p.src_type = AVIRB200_F32;
     p.src_row_base = mid_row_base;
     p.dst = d_dst;
@@ -605,31 +564,6 @@ int shard_compute_axis(const DevAxis& vaxis, int rank, int nranks, avirb200_shar
 
 int shard_compute(const avirb200_plan* pl, int rank, int nranks, avirb200_shard_info* info) {
     return shard_compute_axis(pl->v.hostdev, rank, nranks, info);
-}
-
-// Geometry-only view of an axis descriptor (host pointers), for range arithmetic.
-DevAxis host_axis_view(const avirb200_axis_desc& ad) {
-    DevAxis d;
-    std::memset(&d, 0, sizeof d);
-    d.src_len = ad.src_len; d.dst_len = ad.dst_len; d.nsteps = ad.nsteps;
-    int lo = 0, hi = ad.src_len;
-    for (int i = 0; i < ad.nsteps && i < AVIRB200_MAX_STEPS; ++i) {
-        const avirb200_step_desc& s = ad.steps[i];
-        DevStep& ds = d.steps[i];
-        ds.kind = s.kind; ds.resample = s.resample; ds.latency = s.latency; ds.edge = s.edge;
-        ds.in_len = s.in_len; ds.out_len = s.out_len; ds.ntaps = s.ntaps; ds.order = s.order;
-        ds.upsampled = s.upsampled; ds.skip_odd = s.skip_odd; ds.zero_start = s.zero_start;
-        ds.nphases = s.nphases;
-        ds.out_prefix = s.out_prefix; ds.out_suffix = s.out_suffix;
-        ds.in_prefix = s.in_prefix; ds.in_suffix = s.in_suffix;
-        ds.n_prefix_dc = s.n_prefix_dc; ds.n_suffix_dc = s.n_suffix_dc;
-        ds.in_lo = lo; ds.in_hi = hi;
-        ds.taps = s.taps; ds.src_pos = s.src_pos; ds.phase = s.phase; ds.frac = s.frac;
-        ds.prefix_dc = s.prefix_dc; ds.suffix_dc = s.suffix_dc;
-        const Range od = step_output_domain(ds);
-        lo = od.a; hi = od.b + 1;
-    }
-    return d;
 }
 
 // ---- error-diffusion ditherer (upstream CImageResizerDithererErrdINL / ErrdDIL) ---------------
@@ -818,22 +752,47 @@ __global__ void __launch_bounds__(256) widen_f32_kernel(const float* __restrict_
     dst[(long long)y * dst_pitch + x] = (double)src[i]; // (Tout) v[c], avir.h:3168-3171
 }
 
-size_t f64_in_bytes(const avirb200_plan* pl) {
-    const avirb200_plan_desc& d = pl->desc;
-    return pl->io_in_type == AVIRB200_F64 ? align_up((size_t)d.src_w * d.src_h * d.channels * 4, 256) : 0;
-}
-
-size_t f64_out_bytes(const avirb200_plan* pl) { // float copy of the destination (double output, error diffusion)
-    const avirb200_plan_desc& d = pl->desc;
-    return (pl->io_out_type == AVIRB200_F64 || pl->errd) ? align_up((size_t)d.dst_w * d.dst_h * d.channels * 4, 256) : 0;
-}
-
 // error diffusion: per 32-row group one row of boundary values + one progress counter
 int errd_groups(const avirb200_plan* pl) { return (pl->desc.dst_h + 31) / 32; }
-size_t errd_bytes(const avirb200_plan* pl) {
-    if (!pl->errd) return 0;
+
+// The workspace of one call: byte offsets of its segments, in this order, each 256-byte aligned.
+//   mid        the intermediate: mid_rows rows of mid_pitch() floats (at offset 0)
+//   in32       float copy of a double source                                  } whole-image calls only
+//   out32      float copy of the destination (double output, error diffusion) } (resize_device):
+//   errd_bnd   error diffusion: boundary rows, one per 32-row group           } sharded and per-pass
+//   errd_prog  error diffusion: progress counters                             } calls refuse such plans
+//   src4       the widened source of src_rows rows   } widened plans (pad4) only
+//   dst4       the widened destination of dst_rows rows }
+// Segments a plan does not use are empty.
+struct WsLayout {
+    size_t in32, out32, errd_bnd, errd_prog, src4, dst4, total;
+};
+WsLayout ws_layout(const avirb200_plan* pl, int mid_rows, int src_rows, int dst_rows, bool whole) {
     const avirb200_plan_desc& d = pl->desc;
-    return align_up((size_t)errd_groups(pl) * d.dst_w * d.channels * 4, 256) + align_up((size_t)errd_groups(pl) * 4, 256);
+    const bool f64_in = whole && pl->io_in_type == AVIRB200_F64;
+    const bool f32_out = whole && (pl->io_out_type == AVIRB200_F64 || pl->errd);
+    const bool errd = whole && pl->errd;
+    WsLayout w;
+    size_t off = align_up((size_t)mid_rows * mid_pitch(pl) * sizeof(float), 256);
+    auto seg = [&](bool on, size_t bytes) {
+        const size_t at = off;
+        if (on) off += align_up(bytes, 256);
+        return at;
+    };
+    w.in32 = seg(f64_in, (size_t)d.src_w * d.src_h * d.channels * sizeof(float));
+    w.out32 = seg(f32_out, (size_t)d.dst_w * d.dst_h * d.channels * sizeof(float));
+    w.errd_bnd = seg(errd, (size_t)errd_groups(pl) * d.dst_w * d.channels * sizeof(float));
+    w.errd_prog = seg(errd, (size_t)errd_groups(pl) * sizeof(int));
+    w.src4 = seg(pl->pad4, (size_t)src_rows * d.src_w * 4 * elem_size(d.in_type));
+    w.dst4 = seg(pl->pad4, (size_t)dst_rows * d.dst_w * 4 * elem_size(d.out_type));
+    w.total = off;
+    return w;
+}
+// The whole image's layout (resize_device, the per-pass entry points, the banded host call).
+WsLayout ws_layout(const avirb200_plan* pl) { return ws_layout(pl, pl->desc.src_h, pl->desc.src_h, pl->desc.dst_h, true); }
+// One band of the sharded schedule.
+WsLayout ws_layout(const avirb200_plan* pl, const avirb200_shard_info& si) {
+    return ws_layout(pl, si.need_rows, si.src_rows, si.dst_rows, false);
 }
 
 // ---- host-call staging: one set of device buffers per device, shared by every plan ----------------
@@ -934,7 +893,6 @@ Staging& staging_of(int device) {
     static Staging pool[64];
     return pool[(unsigned)device & 63u];
 }
-int grow(void** p, size_t* have, size_t need);
 int grow(void** p, size_t* have, size_t need) {
     if (*have >= need) return 0;
     cudaFree(*p);
@@ -964,9 +922,29 @@ int plan_staging(avirb200_plan* pl, size_t in_bytes, size_t out_bytes, size_t ws
 // and filters its interior rows meanwhile; before the column pass a one-warp kernel waits for
 // the neighbours' sequence numbers and the rows move from the mailbox into the workspace.
 // Two slots (call parity): a rank can be at most one call ahead of a neighbour, because its
-// column pass needs that neighbour's rows of the same call.
-//   mailbox of rank q:  [256 B: flag_from_up, flag_from_down]
-//                       slot 0: [rows from q-1: halo_up(q)] [rows from q+1: halo_down(q)]   slot 1: the same
+// column pass needs that neighbour's rows of the same call.  avirb200_resize_sharded_local keeps
+// one mailbox per band in one device's memory, with one slot.
+//
+// The mailbox of band q, as MailboxLayout describes it:
+//   [256 B header: flag "from above" at +0, flag "from below" at +4, the sender's counters at +64]
+//   slot 0: [rows from q-1: halo_up(q)] [rows from q+1: halo_down(q), at +align256(up_bytes)]   slot 1: the same
+struct MailboxLayout {
+    static constexpr size_t kHeader = 256, kCounters = 64;
+    size_t up_bytes = 0, down_bytes = 0;
+    MailboxLayout() = default;
+    MailboxLayout(const avirb200_plan* pl, const avirb200_shard_info& si)
+        : up_bytes((size_t)si.halo_up * mid_pitch(pl) * sizeof(float)),
+          down_bytes((size_t)si.halo_down * mid_pitch(pl) * sizeof(float)) {}
+    size_t slot_bytes() const { return align_up(up_bytes, 256) + align_up(down_bytes, 256); }
+    size_t bytes(int slots) const { return kHeader + (size_t)slots * slot_bytes(); }
+    // the mailbox at `box` (this process's address of it), slot `slot`
+    avs::StreamMailbox at(char* box, int slot) const {
+        char* s = box + kHeader + (size_t)slot * slot_bytes();
+        return {reinterpret_cast<float*>(s), reinterpret_cast<float*>(s + align_up(up_bytes, 256)),
+                reinterpret_cast<unsigned*>(box), reinterpret_cast<unsigned long long*>(box + kCounters)};
+    }
+};
+
 struct Halo {
     void* comm = nullptr;
     int rank = -1, nranks = 0;
@@ -974,15 +952,11 @@ struct Halo {
     char* box = nullptr;       // my mailbox
     char* box_up = nullptr;    // rank-1's mailbox, mapped
     char* box_down = nullptr;  // rank+1's mailbox, mapped
-    size_t up_bytes = 0, down_bytes = 0, slot_bytes = 0;             // my own layout
-    size_t nb_up_off = 0, nb_up_slot = 0, nb_up_bytes = 0;           // where my top rows go in rank-1's box
-    size_t nb_down_off = 0, nb_down_slot = 0, nb_down_bytes = 0;     // where my bottom rows go in rank+1's box
+    MailboxLayout mine, above, below; // the layouts of the three
     unsigned long long off_up = 0, off_down = 0; // the neighbours' mailboxes inside their allocations
     unsigned seq = 0;
     unsigned* h_seq = nullptr; // pinned ring of sequence numbers the flag copies read
 };
-
-size_t align256(size_t v) { return (v + 255) / 256 * 256; }
 
 // Waits for the neighbours' sequence numbers, then moves their rows from the mailbox into the
 // workspace (both directions, one launch).
@@ -1058,8 +1032,6 @@ void halo_free(Halo* h) {
     delete h;
 }
 
-int shard_compute(const avirb200_plan* pl, int rank, int nranks, avirb200_shard_info* info);
-
 // Collective over `comm` (every rank of the sharded call makes it): builds and maps the mailboxes.
 // Leaves h->usable false (on EVERY rank) when any rank could not: the NCCL schedule runs then.
 int halo_setup(avirb200_plan* pl, void* comm, int rank, int nranks, cudaStream_t st) {
@@ -1068,35 +1040,24 @@ int halo_setup(avirb200_plan* pl, void* comm, int rank, int nranks, cudaStream_t
     halo_free(pl->halo);
     Halo* h = pl->halo = new Halo();
     h->comm = comm; h->rank = rank; h->nranks = nranks;
-    const size_t rowb = (size_t)pl->desc.dst_w * pl->mid_ch * sizeof(float);
-    auto layout = [&](int q, size_t& upb, size_t& downb, size_t& slotb) -> int {
+    auto layout = [&](int q, MailboxLayout& l) -> int {
         avirb200_shard_info si;
-        int r = shard_compute(pl, q, nranks, &si);
-        if (r != 0) return r;
-        upb = (size_t)si.halo_up * rowb; downb = (size_t)si.halo_down * rowb;
-        slotb = align256(upb) + align256(downb);
-        return 0;
+        const int r = shard_compute(pl, q, nranks, &si);
+        if (r == 0) l = MailboxLayout(pl, si);
+        return r;
     };
-    int r = layout(rank, h->up_bytes, h->down_bytes, h->slot_bytes);
+    int r = layout(rank, h->mine);
+    if (r == 0 && rank > 0) r = layout(rank - 1, h->above);
+    if (r == 0 && rank + 1 < nranks) r = layout(rank + 1, h->below);
     if (r != 0) return r;
     bool ok = nc->AllGather != nullptr;
-    if (rank > 0) {
-        size_t u, d, sl;
-        if ((r = layout(rank - 1, u, d, sl)) != 0) return r;
-        h->nb_up_off = 256 + align256(u); h->nb_up_slot = sl; h->nb_up_bytes = d; // its "from below" area
-    }
-    if (rank + 1 < nranks) {
-        size_t u, d, sl;
-        if ((r = layout(rank + 1, u, d, sl)) != 0) return r;
-        h->nb_down_off = 256; h->nb_down_slot = sl; h->nb_down_bytes = u;          // its "from above" area
-    }
     cudaIpcMemHandle_t mine;
     std::memset(&mine, 0, sizeof mine);
     // its own allocation (the driver carves small requests out of shared blocks, and an IPC handle
     // names the whole block): at least 2 MiB, in multiples of 2 MiB
-    const size_t box_bytes = ((256 + 2 * h->slot_bytes + 256) + (2u << 20) - 1) / (2u << 20) * (2u << 20);
+    const size_t box_bytes = align_up(h->mine.bytes(2), 2u << 20);
     if (ok) ok = cudaMalloc(&h->box, box_bytes) == cudaSuccess;
-    if (ok) ok = cudaMemset(h->box, 0, 256) == cudaSuccess;
+    if (ok) ok = cudaMemset(h->box, 0, MailboxLayout::kHeader) == cudaSuccess;
     if (ok) ok = cudaHostAlloc(&h->h_seq, 64 * sizeof(unsigned), cudaHostAllocPortable) == cudaSuccess;
     if (ok) ok = cudaIpcGetMemHandle(&mine, h->box) == cudaSuccess;
     // (an IPC handle names the allocation the pointer lies in; importers add the pointer's offset in it)
@@ -1167,23 +1128,24 @@ int halo_setup(avirb200_plan* pl, void* comm, int rank, int nranks, cudaStream_t
     return 0;
 }
 
-// Sharded calls: after the row pass (stream st) the first top_rows / last bot_rows rows of the band go to the
-// neighbours' mailboxes on the exchange stream (copy engines), each followed by the call's sequence number.
-int sharded_push(avirb200_plan* pl, Halo* h, cudaStream_t st, const float* own, size_t rowf, int top_rows, int bot_rows,
-                 int src_rows, char* up_dst, char* down_dst, const unsigned* hs) {
+// Sharded calls: after the row pass (stream st) the band's boundary rows go to the neighbours' mailboxes on
+// the exchange stream (copy engines), each followed by the call's sequence number (at hs).
+int sharded_push(avirb200_plan* pl, cudaStream_t st, const float* own, const avs::StreamLink& l, const unsigned* hs) {
+    const size_t rowf = mid_pitch(pl);
+    const int top_rows = avs::stream_rows_up(l), bot_rows = avs::stream_rows_down(l);
     if (pl->stream_x == nullptr) CUDA_TRY(cudaStreamCreateWithFlags(&pl->stream_x, cudaStreamNonBlocking));
     if (pl->ev_x0 == nullptr) CUDA_TRY(cudaEventCreateWithFlags(&pl->ev_x0, cudaEventDisableTiming));
     if (pl->ev_x1 == nullptr) CUDA_TRY(cudaEventCreateWithFlags(&pl->ev_x1, cudaEventDisableTiming));
     CUDA_TRY(cudaEventRecord(pl->ev_x0, st));
     CUDA_TRY(cudaStreamWaitEvent(pl->stream_x, pl->ev_x0, 0));
     if (top_rows > 0) {
-        CUDA_TRY(cudaMemcpyAsync(up_dst, own, (size_t)top_rows * rowf * 4, cudaMemcpyDefault, pl->stream_x));
-        CUDA_TRY(cudaMemcpyAsync(h->box_up + 4, hs, 4, cudaMemcpyDefault, pl->stream_x)); // its flag "from below"
+        CUDA_TRY(cudaMemcpyAsync(l.above.from_dn, own, (size_t)top_rows * rowf * 4, cudaMemcpyDefault, pl->stream_x));
+        CUDA_TRY(cudaMemcpyAsync(&l.above.flags[1], hs, 4, cudaMemcpyDefault, pl->stream_x));
     }
     if (bot_rows > 0) {
-        CUDA_TRY(cudaMemcpyAsync(down_dst, own + (size_t)(src_rows - bot_rows) * rowf, (size_t)bot_rows * rowf * 4,
-                                 cudaMemcpyDefault, pl->stream_x));
-        CUDA_TRY(cudaMemcpyAsync(h->box_down, hs, 4, cudaMemcpyDefault, pl->stream_x));    // its flag "from above"
+        CUDA_TRY(cudaMemcpyAsync(l.below.from_up, own + (size_t)(l.me->src_rows - bot_rows) * rowf,
+                                 (size_t)bot_rows * rowf * 4, cudaMemcpyDefault, pl->stream_x));
+        CUDA_TRY(cudaMemcpyAsync(&l.below.flags[0], hs, 4, cudaMemcpyDefault, pl->stream_x));
     }
     CUDA_TRY(cudaEventRecord(pl->ev_x1, pl->stream_x));
     return 0;
@@ -1348,18 +1310,6 @@ int avirb200_plan_create(const avirb200_plan_desc* desc, avirb200_plan** out) {
     pl->mid_ch = desc->channels;
     fast_plan_init(pl->fast, pl->h.hostdev, pl->v.hostdev, d4);
     // (pl->h.desc / pl->v.desc: the copies whose table pointers stay valid for the plan's life)
-    for (int i = 0; i < pl->h.desc.nsteps; ++i) {
-        avirb200_step_desc& sd = pl->h.desc.steps[i];
-        sd.taps = pl->h.taps[i].data(); sd.src_pos = pl->h.src_pos[i].data();
-        sd.phase = pl->h.phase[i].data(); sd.frac = pl->h.frac[i].data();
-        sd.prefix_dc = pl->h.pdc[i].data(); sd.suffix_dc = pl->h.sdc[i].data();
-    }
-    for (int i = 0; i < pl->v.desc.nsteps; ++i) {
-        avirb200_step_desc& sd = pl->v.desc.steps[i];
-        sd.taps = pl->v.taps[i].data(); sd.src_pos = pl->v.src_pos[i].data();
-        sd.phase = pl->v.phase[i].data(); sd.frac = pl->v.frac[i].data();
-        sd.prefix_dc = pl->v.pdc[i].data(); sd.suffix_dc = pl->v.sdc[i].data();
-    }
     if (avs::stream_row_source_ok(pl->desc))
         avs::stream_plan_axis(pl->h.desc, desc->sum_mode, d4.channels, pl->stream_h, 0, false);
     avs::stream_plan_axis(pl->v.desc, desc->sum_mode, d4.channels, pl->stream_v, 0, true);
@@ -1402,9 +1352,7 @@ void avirb200_plan_destroy(avirb200_plan* pl) {
 
 int avirb200_plan_workspace_bytes(const avirb200_plan* pl, size_t* bytes) {
     if (pl == nullptr || bytes == nullptr) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
-    const avirb200_plan_desc& d = pl->desc;
-    *bytes = align_up((size_t)d.dst_w * d.src_h * pl->mid_ch * sizeof(float), 256) + f64_in_bytes(pl) +
-             f64_out_bytes(pl) + errd_bytes(pl) + pad4_src_bytes(pl, d.src_h) + pad4_dst_bytes(pl, d.dst_h);
+    *bytes = ws_layout(pl).total;
     return 0;
 }
 
@@ -1424,14 +1372,10 @@ int avirb200_resize_device(const avirb200_plan* pl, const void* d_src, size_t sr
     }
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     int launches = 0;
-    // double buffers: float copies live behind the intermediate in the workspace
     char* wsb = static_cast<char*>(d_ws);
-    float* in32 = reinterpret_cast<float*>(wsb + align_up((size_t)d.dst_w * d.src_h * pl->mid_ch * 4, 256));
-    // (1..3-channel plans on the 4-channel kernels have no double buffers / error diffusion: their
-    // scratch copies start where in32 would)
-    char* src4 = reinterpret_cast<char*>(in32);
-    char* dst4 = src4 + pad4_src_bytes(pl, d.src_h);
-    float* out32 = reinterpret_cast<float*>(reinterpret_cast<char*>(in32) + f64_in_bytes(pl));
+    const WsLayout ws = ws_layout(pl);
+    float* in32 = reinterpret_cast<float*>(wsb + ws.in32);
+    float* out32 = reinterpret_cast<float*>(wsb + ws.out32);
     const void* ksrc = d_src;
     size_t ksrc_pitch = src_pitch;
     void* kdst = d_dst;
@@ -1449,10 +1393,10 @@ int avirb200_resize_device(const avirb200_plan* pl, const void* d_src, size_t sr
         kdst = out32;
         kdst_pitch = (size_t)d.dst_w * d.channels;
     }
-    int r = run_row_pass(pl, ksrc, ksrc_pitch, static_cast<float*>(d_ws), d.src_h, st, &launches, src4);
+    int r = run_row_pass(pl, ksrc, ksrc_pitch, static_cast<float*>(d_ws), d.src_h, st, &launches, wsb + ws.src4);
     if (r != 0) return r;
     r = run_col_pass(pl, static_cast<const float*>(d_ws), 0, kdst, kdst_pitch, 0, d.dst_h, st,
-                     &launches, dst4);
+                     &launches, wsb + ws.dst4);
     if (r == 0 && pl->io_out_type == AVIRB200_F64) {
         const int re = d.dst_w * d.channels;
         const long long n = (long long)re * d.dst_h;
@@ -1471,9 +1415,8 @@ int avirb200_resize_device(const avirb200_plan* pl, const void* d_src, size_t sr
         ep.round_mode = d.round_mode;
         ep.planar = (d.sum_mode == AVIRB200_SUM_DIL8) ? 1 : 0;
         ep.tr_mul = d.tr_mul; ep.tr_mul_inv = d.tr_mul_inv; ep.pk_out = d.pk_out;
-        char* eb = reinterpret_cast<char*>(out32) + f64_out_bytes(pl);
-        ep.boundary = reinterpret_cast<float*>(eb);
-        ep.progress = reinterpret_cast<int*>(eb + align_up((size_t)errd_groups(pl) * d.dst_w * d.channels * 4, 256));
+        ep.boundary = reinterpret_cast<float*>(wsb + ws.errd_bnd);
+        ep.progress = reinterpret_cast<int*>(wsb + ws.errd_prog);
         CUDA_TRY(cudaMemsetAsync(ep.progress, 0, (size_t)errd_groups(pl) * 4, st));
         switch (d.channels) {
         case 1: errd_kernel<1><<<errd_groups(pl), 32, 0, st>>>(ep); break;
@@ -1494,10 +1437,8 @@ int avirb200_row_pass_device(const avirb200_plan* pl, const void* d_src, size_t 
         return fail(AVIRB200_ERR_BAD_ARG, "null argument");
     if (plan_has_f64(pl)) return fail(AVIRB200_ERR_UNSUPPORTED, "per-pass entry points: no double buffers, no error diffusion");
     int launches = 0;
-    const avirb200_plan_desc& d = pl->desc;
-    char* src4 = static_cast<char*>(d_ws) + align_up((size_t)d.dst_w * d.src_h * pl->mid_ch * 4, 256);
     return run_row_pass(pl, d_src, src_pitch, static_cast<float*>(d_ws), pl->desc.src_h,
-                        static_cast<cudaStream_t>(stream), &launches, src4);
+                        static_cast<cudaStream_t>(stream), &launches, static_cast<char*>(d_ws) + ws_layout(pl).src4);
 }
 
 int avirb200_col_pass_device(const avirb200_plan* pl, const void* d_ws, void* d_dst,
@@ -1506,11 +1447,9 @@ int avirb200_col_pass_device(const avirb200_plan* pl, const void* d_ws, void* d_
         return fail(AVIRB200_ERR_BAD_ARG, "null argument");
     if (plan_has_f64(pl)) return fail(AVIRB200_ERR_UNSUPPORTED, "per-pass entry points: no double buffers, no error diffusion");
     int launches = 0;
-    const avirb200_plan_desc& d = pl->desc;
-    char* dst4 = static_cast<char*>(const_cast<void*>(d_ws)) + align_up((size_t)d.dst_w * d.src_h * pl->mid_ch * 4, 256) +
-                 pad4_src_bytes(pl, d.src_h);
-    return run_col_pass(pl, static_cast<const float*>(d_ws), 0, d_dst, dst_pitch, 0,
-                        pl->desc.dst_h, static_cast<cudaStream_t>(stream), &launches, dst4);
+    return run_col_pass(pl, static_cast<const float*>(d_ws), 0, d_dst, dst_pitch, 0, pl->desc.dst_h,
+                        static_cast<cudaStream_t>(stream), &launches,
+                        static_cast<char*>(const_cast<void*>(d_ws)) + ws_layout(pl).dst4);
 }
 
 int avirb200_resize_device_batch(const avirb200_plan* pl, int n, const void* const* d_srcs, size_t src_pitch,
@@ -1548,8 +1487,8 @@ int avirb200_resize_host(avirb200_plan* pl, const void* h_src, size_t src_pitch,
         }
     }
     std::lock_guard<std::mutex> sl(staging_of(pl->device).mx);
-    const size_t in_row = (size_t)d.src_w * d.channels * dtype_size(pl->io_in_type);
-    const size_t out_row = (size_t)d.dst_w * d.channels * dtype_size(pl->io_out_type);
+    const size_t in_row = (size_t)d.src_w * d.channels * elem_size(pl->io_in_type);
+    const size_t out_row = (size_t)d.dst_w * d.channels * elem_size(pl->io_out_type);
     const size_t in_bytes = in_row * d.src_h, out_bytes = out_row * d.dst_h;
     size_t ws = 0;
     avirb200_plan_workspace_bytes(pl, &ws);
@@ -1558,7 +1497,7 @@ int avirb200_resize_host(avirb200_plan* pl, const void* h_src, size_t src_pitch,
         const int r0 = plan_staging(pl, in_bytes, out_bytes, ws);
         if (r0 != 0) return r0;
     }
-    const size_t in_el = dtype_size(pl->io_in_type), out_el = dtype_size(pl->io_out_type);
+    const size_t in_el = elem_size(pl->io_in_type), out_el = elem_size(pl->io_out_type);
     // Pipelined form for large images: the image is cut into row bands (the multi-GPU band
     // arithmetic, one shared intermediate buffer instead of a halo exchange).  Band b's rows
     // travel host->device on the copy-in stream while the kernels of band b-1 run on the
@@ -1595,10 +1534,10 @@ int avirb200_resize_host(avirb200_plan* pl, const void* h_src, size_t src_pitch,
             CUDA_TRY(cudaEventCreateWithFlags(&e1, cudaEventDisableTiming));
             pl->ev_out.push_back(e1);
         }
-        const size_t rowf = (size_t)d.dst_w * pl->mid_ch;
+        const size_t rowf = mid_pitch(pl);
         const size_t dsrc_pitch = (size_t)d.src_w * d.channels, ddst_pitch = (size_t)d.dst_w * d.channels;
-        char* src4 = static_cast<char*>(pl->d_ws) + align_up((size_t)d.dst_w * d.src_h * pl->mid_ch * 4, 256);
-        char* dst4 = src4 + pad4_src_bytes(pl, d.src_h);
+        char* src4 = static_cast<char*>(pl->d_ws) + ws_layout(pl).src4;
+        char* dst4 = static_cast<char*>(pl->d_ws) + ws_layout(pl).dst4;
         const size_t src4_row = (size_t)d.src_w * 4 * in_el, dst4_row = (size_t)d.dst_w * 4 * out_el;
         int launches = 0;
         // Pageable (malloc) caller buffers: a copy call straight from / to them returns only when
@@ -1726,8 +1665,7 @@ int avirb200_shard_workspace_bytes(const avirb200_plan* pl, int rank, int nranks
     int r = shard_compute(pl, rank, nranks, &si);
     if (r != 0) return r;
     fast_prepare_range(pl->fast, si.dst_row0, si.dst_row0 + si.dst_rows);
-    *bytes = align_up((size_t)si.need_rows * pl->desc.dst_w * pl->mid_ch * sizeof(float), 256) +
-             pad4_src_bytes(pl, si.src_rows) + pad4_dst_bytes(pl, si.dst_rows);
+    *bytes = ws_layout(pl, si).total;
     return 0;
 }
 
@@ -1765,12 +1703,13 @@ int avirb200_resize_sharded(const avirb200_plan* cpl, void* comm, int rank, int 
     if (r != 0) return r;
     const avirb200_plan_desc& d = pl->desc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const size_t rowf = (size_t)d.dst_w * pl->mid_ch; // floats per intermediate row
-    const size_t in_el = dtype_size(d.in_type);
+    const size_t rowf = mid_pitch(pl);
+    const size_t in_el = elem_size(d.in_type);
     float* mid = static_cast<float*>(d_ws);
     float* own = mid + (size_t)si.halo_up * rowf;
-    char* src4 = static_cast<char*>(d_ws) + align_up((size_t)si.need_rows * rowf * sizeof(float), 256);
-    char* dst4 = src4 + pad4_src_bytes(pl, si.src_rows);
+    const WsLayout ws = ws_layout(pl, si);
+    char* src4 = static_cast<char*>(d_ws) + ws.src4;
+    char* dst4 = static_cast<char*>(d_ws) + ws.dst4;
     const size_t src4_row = (size_t)d.src_w * 4 * in_el;
     int launches = 0;
     if (nranks <= 1) {
@@ -1789,8 +1728,11 @@ int avirb200_resize_sharded(const avirb200_plan* cpl, void* comm, int rank, int 
     std::memset(&up, 0, sizeof up); std::memset(&down, 0, sizeof down);
     if (rank > 0) { r = shard_compute(pl, rank - 1, nranks, &up); if (r != 0) return r; }
     if (rank + 1 < nranks) { r = shard_compute(pl, rank + 1, nranks, &down); if (r != 0) return r; }
-    const int top_rows = (rank > 0) ? up.halo_down : 0;              // my first rows go up
-    const int bot_rows = (rank + 1 < nranks) ? down.halo_up : 0;     // my last rows go down
+    avs::StreamLink link; // (the mailboxes are filled in below)
+    link.me = &si;
+    link.up = (rank > 0) ? &up : nullptr;
+    link.dn = (rank + 1 < nranks) ? &down : nullptr;
+    const int top_rows = avs::stream_rows_up(link), bot_rows = avs::stream_rows_down(link);
 
     std::lock_guard<std::mutex> lk(pl->mx);
     if (pl->opt_overlap) {
@@ -1811,54 +1753,30 @@ int avirb200_resize_sharded(const avirb200_plan* cpl, void* comm, int rank, int 
             return run_row_pass(pl, srcb + (size_t)row0 * src_pitch * in_el, src_pitch, own + (size_t)row0 * rowf,
                                 nrows, st, &launches, src4 + (size_t)row0 * src4_row);
         };
-        const int need_up = (rank > 0 && si.halo_up > 0) ? 1 : 0;
-        const int need_down = (rank + 1 < nranks && si.halo_down > 0) ? 1 : 0;
-        char* const up_dst = h->box_up + h->nb_up_off + (size_t)slot * h->nb_up_slot;         // my first rows, in rank-1's mailbox
-        char* const down_dst = h->box_down + h->nb_down_off + (size_t)slot * h->nb_down_slot; // my last rows, in rank+1's
-        const char* const my_slot = h->box + 256 + (size_t)slot * h->slot_bytes;
+        const int need_up = (link.up && si.halo_up > 0) ? 1 : 0;
+        const int need_down = (link.dn && si.halo_down > 0) ? 1 : 0;
+        link.seq = seq;
+        link.mine = h->mine.at(h->box, slot);
+        if (link.up) link.above = h->above.at(h->box_up, slot);
+        if (link.dn) link.below = h->below.at(h->box_down, slot);
         // AVIRB200_OPT_OVERLAP_HALO = 3, the fused exchange: the row kernel stores the rows the neighbours need
         // into their mailboxes as it produces them (peer stores over NVLink) and raises their flags when the
         // last of them is out; the column kernel reads the neighbours' rows in place from this rank's mailbox,
         // waiting on the flags only in the runs that touch them.  No exchange stream, no copy, no extra launch.
         // Either half falls back on its own (the mailbox protocol is the same): a row pass that is not on the
         // streaming kernel pushes with the copy engines, a column pass that is not pulls into the workspace.
-        // (Slots alternate per call and are reused two calls later; what orders the reuse is that a rank's
-        // call n+1 needs its neighbour's call-n+1 rows, sent after the neighbour's call-n column pass: so the
-        // fused halves run only between neighbours that exchange rows in BOTH directions.)
-        const bool both_ways = (rank == 0 || ((top_rows > 0) == (si.halo_up > 0))) &&
-                               (rank + 1 >= nranks || ((bot_rows > 0) == (si.halo_down > 0)));
-        const bool fused = pl->opt_overlap == 3 && both_ways;
-        // (the fused sender keeps one mailbox per 16-line strip: not for bands so short that a strip holds
-        // rows of both neighbours)
-        const bool fused_tx = fused && !(top_rows > 0 && bot_rows > 0 && (top_rows + 15) / 16 > (si.src_rows - bot_rows) / 16);
+        const bool fused = pl->opt_overlap == 3 && avs::stream_fused_rx_ok(link);
+        const bool fused_tx = pl->opt_overlap == 3 && avs::stream_fused_tx_ok(link);
         bool sent = false, pushed = false;
         if (fused_tx && top_rows + bot_rows > 0) {
-            avs::StreamParams xs;
-            std::memset(&xs, 0, sizeof xs);
-            const int L = 16; // lines of a strip (avs::kLines)
-            xs.xs_seq = seq;
-            xs.xs_count = reinterpret_cast<unsigned long long*>(h->box + 64);
-            if (top_rows > 0) {
-                xs.xs_up_dst = reinterpret_cast<float*>(up_dst);
-                xs.xs_up_flag = reinterpret_cast<unsigned*>(h->box_up + 4); // its flag "from below"
-                xs.xs_top = top_rows;
-                xs.xs_units[0] = (unsigned long long)((top_rows + L - 1) / L);
-            }
-            if (bot_rows > 0) {
-                xs.xs_dn_dst = reinterpret_cast<float*>(down_dst);
-                xs.xs_dn_flag = reinterpret_cast<unsigned*>(h->box_down); // its flag "from above"
-                xs.xs_bot0 = si.src_rows - bot_rows;
-                xs.xs_bot = bot_rows;
-                xs.xs_units[1] = (unsigned long long)((si.src_rows + L - 1) / L - xs.xs_bot0 / L);
-            }
-            if ((r = run_row_pass(pl, d_src, src_pitch, own, si.src_rows, st, &launches, src4, 0, 0, &xs, &sent)) != 0) return r;
+            if ((r = run_row_pass(pl, d_src, src_pitch, own, si.src_rows, st, &launches, src4, 0, 0, &link, &sent)) != 0) return r;
         } else {
             // 1. the rows the neighbours need (one launch on the streaming kernel: two line segments),
             // 2. their push on the exchange stream, 3. the interior rows
             // (boundary rows first only on request, AVIRB200_OPT_OVERLAP_HALO = 2: the copy-engine push
             // of cfg3's 1.2 MB is short next to the extra launch the split costs)
             const bool split = pl->opt_overlap == 2 && top_rows + bot_rows < si.src_rows;
-            if (split && row_pass_can_segment(pl, d_src, src_pitch, own)) {
+            if (split && !use_pad4(pl) && row_pass_on_stream(pl, d_src, src_pitch, own)) {
                 if (top_rows + bot_rows > 0 &&
                     (r = run_row_pass(pl, d_src, src_pitch, own, si.src_rows, st, &launches, nullptr, top_rows, bot_rows)) != 0)
                     return r;
@@ -1868,38 +1786,30 @@ int avirb200_resize_sharded(const avirb200_plan* cpl, void* comm, int rank, int 
             } else if ((r = rows_pass(0, si.src_rows)) != 0) {
                 return r;
             }
-            if ((r = sharded_push(pl, h, st, own, rowf, top_rows, bot_rows, si.src_rows, up_dst, down_dst, hs)) != 0) return r;
+            if ((r = sharded_push(pl, st, own, link, hs)) != 0) return r;
             sent = pushed = true;
             if (split && (r = rows_pass(top_rows, si.src_rows - top_rows - bot_rows)) != 0) return r;
         }
         if (!sent && top_rows + bot_rows > 0) { // the fused row pass did not run on the streaming kernel
-            if ((r = sharded_push(pl, h, st, own, rowf, top_rows, bot_rows, si.src_rows, up_dst, down_dst, hs)) != 0) return r;
+            if ((r = sharded_push(pl, st, own, link, hs)) != 0) return r;
             pushed = true;
         }
         // 4. the neighbours' rows: in place (fused), or wait for their sequence numbers and move them
         // mailbox -> workspace
         r = 1;
         if (fused && (need_up || need_down)) {
-            avs::StreamParams xr;
-            std::memset(&xr, 0, sizeof xr);
-            xr.xr_up_src = reinterpret_cast<const float*>(my_slot);
-            xr.xr_dn_src = reinterpret_cast<const float*>(my_slot + align256(h->up_bytes));
-            xr.xr_flags = reinterpret_cast<const volatile unsigned*>(h->box);
-            xr.xr_seq = seq;
-            xr.xr_own_lo = si.src_row0;
-            xr.xr_own_hi = si.src_row0 + si.src_rows;
             r = run_col_pass(pl, mid, si.need_row0, d_dst, dst_pitch, si.dst_row0, si.dst_row0 + si.dst_rows, st, &launches,
-                             dst4, si.need_rows, &xr);
+                             dst4, si.need_rows, &link);
         }
         if (r == 1) {
             if (need_up || need_down) {
                 (void)cudaGetLastError();
-                halo_pull_kernel<<<64, 256, 0, st>>>(reinterpret_cast<const volatile unsigned*>(h->box), seq, need_up, need_down,
-                                                     reinterpret_cast<const float4*>(my_slot), reinterpret_cast<float4*>(mid),
-                                                     need_up ? h->up_bytes / 16 : 0,
-                                                     reinterpret_cast<const float4*>(my_slot + align256(h->up_bytes)),
+                halo_pull_kernel<<<64, 256, 0, st>>>(link.mine.flags, seq, need_up, need_down,
+                                                     reinterpret_cast<const float4*>(link.mine.from_up), reinterpret_cast<float4*>(mid),
+                                                     need_up ? h->mine.up_bytes / 16 : 0,
+                                                     reinterpret_cast<const float4*>(link.mine.from_dn),
                                                      reinterpret_cast<float4*>(own + (size_t)si.src_rows * rowf),
-                                                     need_down ? h->down_bytes / 16 : 0);
+                                                     need_down ? h->mine.down_bytes / 16 : 0);
                 ++launches;
                 CUDA_TRY(cudaGetLastError());
             }
@@ -1942,8 +1852,8 @@ int avirb200_resize_sharded_host(avirb200_plan* pl, void* comm, int rank, int nr
     if (r != 0) return r;
     size_t ws = 0;
     if ((r = avirb200_shard_workspace_bytes(pl, rank, nranks, &ws)) != 0) return r;
-    const size_t in_row = (size_t)d.src_w * d.channels * dtype_size(d.in_type);
-    const size_t out_row = (size_t)d.dst_w * d.channels * dtype_size(d.out_type);
+    const size_t in_row = (size_t)d.src_w * d.channels * elem_size(d.in_type);
+    const size_t out_row = (size_t)d.dst_w * d.channels * elem_size(d.out_type);
     {
         std::lock_guard<std::mutex> lk(pl->mx);
         int cur = -1;
@@ -1954,12 +1864,12 @@ int avirb200_resize_sharded_host(avirb200_plan* pl, void* comm, int rank, int nr
     std::lock_guard<std::mutex> sl(staging_of(pl->device).mx);
     r = plan_staging(pl, in_row * si.src_rows, out_row * si.dst_rows, ws);
     if (r != 0) return r;
-    CUDA_TRY(cudaMemcpy2DAsync(pl->d_src, in_row, h_src, src_pitch * dtype_size(d.in_type), in_row, si.src_rows,
+    CUDA_TRY(cudaMemcpy2DAsync(pl->d_src, in_row, h_src, src_pitch * elem_size(d.in_type), in_row, si.src_rows,
                                cudaMemcpyHostToDevice, pl->stream));
     r = avirb200_resize_sharded(pl, comm, rank, nranks, pl->d_src, (size_t)d.src_w * d.channels, pl->d_dst,
                                 (size_t)d.dst_w * d.channels, pl->d_ws, pl->stream);
     if (r != 0) return r;
-    CUDA_TRY(cudaMemcpy2DAsync(h_dst, dst_pitch * dtype_size(d.out_type), pl->d_dst, out_row, out_row, si.dst_rows,
+    CUDA_TRY(cudaMemcpy2DAsync(h_dst, dst_pitch * elem_size(d.out_type), pl->d_dst, out_row, out_row, si.dst_rows,
                                cudaMemcpyDeviceToHost, pl->stream));
     CUDA_TRY(cudaStreamSynchronize(pl->stream));
     return 0;
@@ -1973,83 +1883,69 @@ int avirb200_resize_sharded_local(const avirb200_plan* pl, int nranks, const voi
     if (plan_has_f64(pl)) return fail(AVIRB200_ERR_UNSUPPORTED, "sharded calls: no double buffers, no error diffusion");
     const avirb200_plan_desc& d = pl->desc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const size_t rowf = (size_t)d.dst_w * pl->mid_ch;
+    const size_t rowf = mid_pitch(pl);
+    const size_t in_el = elem_size(d.in_type), out_el = elem_size(d.out_type);
     std::vector<avirb200_shard_info> si(nranks);
-    std::vector<float*> mid(nranks);
-    std::vector<char*> src4(nranks), dst4(nranks);
+    std::vector<float*> mid(nranks), own(nranks);
+    std::vector<const char*> src(nranks);
+    std::vector<char*> dst(nranks), src4(nranks), dst4(nranks);
     char* base = static_cast<char*>(d_ws);
     for (int r = 0; r < nranks; ++r) { // every band's segment: as avirb200_shard_workspace_bytes lays it out
         int e = shard_compute(pl, r, nranks, &si[r]);
         if (e != 0) return e;
+        const WsLayout ws = ws_layout(pl, si[r]);
         mid[r] = reinterpret_cast<float*>(base);
-        src4[r] = base + align_up((size_t)si[r].need_rows * rowf * sizeof(float), 256);
-        dst4[r] = src4[r] + pad4_src_bytes(pl, si[r].src_rows);
-        base = dst4[r] + pad4_dst_bytes(pl, si[r].dst_rows);
+        own[r] = mid[r] + (size_t)si[r].halo_up * rowf;
+        src4[r] = base + ws.src4;
+        dst4[r] = base + ws.dst4;
+        base += ws.total;
+        src[r] = static_cast<const char*>(d_src) + (size_t)si[r].src_row0 * src_pitch * in_el;
+        dst[r] = static_cast<char*>(d_dst) + (size_t)si[r].dst_row0 * dst_pitch * out_el;
     }
     int launches = 0;
-    const size_t in_el = dtype_size(d.in_type), out_el = dtype_size(d.out_type);
     // The fused halo exchange of avirb200_resize_sharded (AVIRB200_OPT_OVERLAP_HALO = 3), with every band's
-    // mailbox in this device's memory: the same two kernels, parameters and protocol as between ranks.
-    bool fused = pl->opt_overlap == 3 && nranks > 1 && pl->opt_family == 0 && pl->stream_h.chain != 0 &&
-                 pl->stream_v.chain != 0 && (src_pitch % 4) == 0 && (dst_pitch % 2) == 0 &&
-                 (use_pad4(pl) || ((uintptr_t)d_src % (4 * in_el)) == 0) &&
-                 (use_pad4(pl) || ((uintptr_t)d_dst % (2 * fast_elsize(d.out_type))) == 0);
+    // mailbox (one slot) in this device's memory: the same two kernels, parameters and protocol as between
+    // ranks.  Only when every band may run both fused halves and both its passes run on the streaming kernel
+    // (a widened plan's kernels see its scratch copies).
+    const bool p4 = use_pad4(pl);
+    std::vector<avs::StreamLink> link(nranks);
+    std::vector<MailboxLayout> box(nranks);
     std::vector<size_t> box_off(nranks + 1, 0);
+    bool fused = pl->opt_overlap == 3 && nranks > 1;
     for (int r = 0; r < nranks && fused; ++r) {
-        const int top = (r > 0) ? si[r - 1].halo_down : 0, bot = (r + 1 < nranks) ? si[r + 1].halo_up : 0;
-        if ((r > 0 && (top > 0) != (si[r].halo_up > 0)) || (r + 1 < nranks && (bot > 0) != (si[r].halo_down > 0)) ||
-            (top > 0 && bot > 0 && (top + 15) / 16 > (si[r].src_rows - bot) / 16) || top > si[r].src_rows || bot > si[r].src_rows)
-            fused = false;
-        box_off[r + 1] = box_off[r] + 256 + align256((size_t)si[r].halo_up * rowf * 4) + align256((size_t)si[r].halo_down * rowf * 4);
+        link[r].me = &si[r];
+        if (r > 0) link[r].up = &si[r - 1];
+        if (r + 1 < nranks) link[r].dn = &si[r + 1];
+        fused = avs::stream_fused_tx_ok(link[r]) &&
+                row_pass_on_stream(pl, p4 ? src4[r] : src[r], p4 ? (size_t)d.src_w * 4 : src_pitch, own[r]) &&
+                col_pass_on_stream(pl, p4 ? dst4[r] : dst[r], p4 ? (size_t)d.dst_w * 4 : dst_pitch, mid[r]);
+        box[r] = MailboxLayout(pl, si[r]);
+        box_off[r + 1] = box_off[r] + box[r].bytes(1);
     }
     if (fused) {
         char* boxes = nullptr;
         CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&boxes), box_off[nranks], st));
-        auto box = [&](int r) { return boxes + box_off[r]; };
-        auto box_up_area = [&](int r) { return box(r) + 256; };
-        auto box_dn_area = [&](int r) { return box(r) + 256 + align256((size_t)si[r].halo_up * rowf * 4); };
         int e = 0;
-        for (int r = 0; r < nranks && e == 0; ++r)
-            if (cudaMemsetAsync(box(r), 0, 256, st) != cudaSuccess) e = fail(AVIRB200_ERR_CUDA, "sharded_local: mailbox header");
-        const unsigned seq = 1;
-        for (int r = 0; r < nranks && e == 0; ++r) {
-            float* own = mid[r] + (size_t)si[r].halo_up * rowf;
-            const char* src = static_cast<const char*>(d_src) + (size_t)si[r].src_row0 * src_pitch * in_el;
-            const int top = (r > 0) ? si[r - 1].halo_down : 0, bot = (r + 1 < nranks) ? si[r + 1].halo_up : 0;
-            avs::StreamParams xs;
-            std::memset(&xs, 0, sizeof xs);
-            xs.xs_seq = seq;
-            xs.xs_count = reinterpret_cast<unsigned long long*>(box(r) + 64);
-            if (top > 0) {
-                xs.xs_up_dst = reinterpret_cast<float*>(box_dn_area(r - 1));
-                xs.xs_up_flag = reinterpret_cast<unsigned*>(box(r - 1) + 4);
-                xs.xs_top = top;
-                xs.xs_units[0] = (unsigned long long)((top + 15) / 16);
-            }
-            if (bot > 0) {
-                xs.xs_dn_dst = reinterpret_cast<float*>(box_up_area(r + 1));
-                xs.xs_dn_flag = reinterpret_cast<unsigned*>(box(r + 1));
-                xs.xs_bot0 = si[r].src_rows - bot;
-                xs.xs_bot = bot;
-                xs.xs_units[1] = (unsigned long long)((si[r].src_rows + 15) / 16 - xs.xs_bot0 / 16);
-            }
-            bool sent = false;
-            e = run_row_pass(pl, src, src_pitch, own, si[r].src_rows, st, &launches, src4[r], 0, 0,
-                             (top + bot > 0) ? &xs : nullptr, &sent);
-            if (e == 0 && top + bot > 0 && !sent) e = fail(AVIRB200_ERR_CUDA, "sharded_local: the streaming row pass did not take the band");
+        for (int r = 0; r < nranks; ++r) {
+            link[r].mine = box[r].at(boxes + box_off[r], 0);
+            link[r].seq = 1;
+            if (e == 0 && cudaMemsetAsync(boxes + box_off[r], 0, MailboxLayout::kHeader, st) != cudaSuccess)
+                e = fail(AVIRB200_ERR_CUDA, "sharded_local: mailbox header");
+        }
+        for (int r = 0; r < nranks; ++r) {
+            if (r > 0) link[r].above = link[r - 1].mine;
+            if (r + 1 < nranks) link[r].below = link[r + 1].mine;
         }
         for (int r = 0; r < nranks && e == 0; ++r) {
-            char* dst = static_cast<char*>(d_dst) + (size_t)si[r].dst_row0 * dst_pitch * out_el;
-            avs::StreamParams xr;
-            std::memset(&xr, 0, sizeof xr);
-            xr.xr_up_src = reinterpret_cast<const float*>(box_up_area(r));
-            xr.xr_dn_src = reinterpret_cast<const float*>(box_dn_area(r));
-            xr.xr_flags = reinterpret_cast<const volatile unsigned*>(box(r));
-            xr.xr_seq = seq;
-            xr.xr_own_lo = si[r].src_row0;
-            xr.xr_own_hi = si[r].src_row0 + si[r].src_rows;
-            e = run_col_pass(pl, mid[r], si[r].need_row0, dst, dst_pitch, si[r].dst_row0, si[r].dst_row0 + si[r].dst_rows, st,
-                             &launches, dst4[r], si[r].need_rows, &xr);
+            const bool tx = avs::stream_rows_up(link[r]) + avs::stream_rows_down(link[r]) > 0;
+            bool sent = false;
+            e = run_row_pass(pl, src[r], src_pitch, own[r], si[r].src_rows, st, &launches, src4[r], 0, 0,
+                             tx ? &link[r] : nullptr, &sent);
+            if (e == 0 && tx && !sent) e = fail(AVIRB200_ERR_CUDA, "sharded_local: the streaming row pass did not take the band");
+        }
+        for (int r = 0; r < nranks && e == 0; ++r) {
+            e = run_col_pass(pl, mid[r], si[r].need_row0, dst[r], dst_pitch, si[r].dst_row0, si[r].dst_row0 + si[r].dst_rows,
+                             st, &launches, dst4[r], si[r].need_rows, &link[r]);
             if (e == 1) e = fail(AVIRB200_ERR_CUDA, "sharded_local: the streaming column pass did not take the band");
         }
         cudaFreeAsync(boxes, st);
@@ -2057,27 +1953,22 @@ int avirb200_resize_sharded_local(const avirb200_plan* pl, int nranks, const voi
         return e;
     }
     for (int r = 0; r < nranks; ++r) { // every band's row pass
-        float* own = mid[r] + (size_t)si[r].halo_up * rowf;
-        const char* src = static_cast<const char*>(d_src) + (size_t)si[r].src_row0 * src_pitch * in_el;
-        int e = run_row_pass(pl, src, src_pitch, own, si[r].src_rows, st, &launches, src4[r]);
+        int e = run_row_pass(pl, src[r], src_pitch, own[r], si[r].src_rows, st, &launches, src4[r]);
         if (e != 0) return e;
     }
     for (int r = 0; r < nranks; ++r) { // the "exchange"
-        float* own = mid[r] + (size_t)si[r].halo_up * rowf;
         if (r > 0 && si[r].halo_up > 0) {
-            const float* nb = mid[r - 1] + (size_t)(si[r - 1].halo_up + si[r - 1].src_rows - si[r].halo_up) * rowf;
+            const float* nb = own[r - 1] + (size_t)(si[r - 1].src_rows - si[r].halo_up) * rowf;
             CUDA_TRY(cudaMemcpyAsync(mid[r], nb, (size_t)si[r].halo_up * rowf * 4,
                                      cudaMemcpyDeviceToDevice, st));
         }
         if (r + 1 < nranks && si[r].halo_down > 0) {
-            const float* nb = mid[r + 1] + (size_t)si[r + 1].halo_up * rowf;
-            CUDA_TRY(cudaMemcpyAsync(own + (size_t)si[r].src_rows * rowf, nb,
+            CUDA_TRY(cudaMemcpyAsync(own[r] + (size_t)si[r].src_rows * rowf, own[r + 1],
                                      (size_t)si[r].halo_down * rowf * 4, cudaMemcpyDeviceToDevice, st));
         }
     }
     for (int r = 0; r < nranks; ++r) {
-        char* dst = static_cast<char*>(d_dst) + (size_t)si[r].dst_row0 * dst_pitch * out_el;
-        int e = run_col_pass(pl, mid[r], si[r].need_row0, dst, dst_pitch, si[r].dst_row0,
+        int e = run_col_pass(pl, mid[r], si[r].need_row0, dst[r], dst_pitch, si[r].dst_row0,
                              si[r].dst_row0 + si[r].dst_rows, st, &launches, dst4[r], si[r].need_rows);
         if (e != 0) return e;
     }

@@ -190,14 +190,12 @@ inline bool fast_build_axis(FastPass& fp, const DevAxis& host, int sum_mode) {
     return true;
 }
 
-inline size_t fa_align(size_t v) { return (v + 255) / 256 * 256; }
-
 inline int fast_upload(FastPass& fp) {
     size_t bytes = 0;
     const int ns = fp.hax.nsteps;
     for (int i = 0; i < ns; ++i)
-        bytes += fa_align(fp.eff_taps[i].size() * 4) + fa_align(fp.eff_idx[i].size() * 4) +
-                 fa_align(fp.src_pos[i].size() * 4);
+        bytes += align_up(fp.eff_taps[i].size() * 4, 256) + align_up(fp.eff_idx[i].size() * 4, 256) +
+                 align_up(fp.src_pos[i].size() * 4, 256);
     if (cudaMalloc(&fp.arena, bytes + 256) != cudaSuccess) return -1;
     std::vector<char> img(bytes + 256, 0);
     size_t off = 0;
@@ -208,7 +206,7 @@ inline int fast_upload(FastPass& fp) {
             if (n == 0) return nullptr;
             memcpy(img.data() + off, src, n);
             const void* d = base + off;
-            off += fa_align(n);
+            off += align_up(n, 256);
             return d;
         };
         fp.ax.s[i].taps = static_cast<const float*>(put(fp.eff_taps[i].data(), fp.eff_taps[i].size() * 4));
@@ -279,23 +277,13 @@ inline void fast_fill_common(FastParams& p, const avirb200_plan_desc& d, const f
     p.pk_out = d.pk_out;
 }
 
-inline int fast_sm_count() {
-    static const int sms = [] {
-        int d = 0, n = 0;
-        cudaGetDevice(&d);
-        cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, d);
-        return n > 0 ? n : 1;
-    }();
-    return sms;
-}
-
-// Persistent launch: kFastBlocksPerSM blocks per SM (or fewer when there are fewer tiles).
-inline int fast_launch(const FastParams& p, size_t smem, int sum_mode, cudaStream_t st) {
+// Persistent launch: kFastBlocksPerSM blocks per SM of the plan's device (or fewer when there are fewer tiles).
+inline int fast_launch(const FastParams& p, size_t smem, int sum_mode, int sm_count, cudaStream_t st) {
     const long long tiles = (long long)((p.out1 - p.out0 + p.tile_out - 1) / p.tile_out) *
                             ((p.n_lines + kFastLines - 1) / kFastLines);
     if (tiles <= 0) return 0;
     if (tiles > 0x7fffffffLL) return -2;
-    const long long slots = (long long)fast_sm_count() * kFastBlocksPerSM;
+    const long long slots = (long long)sm_count * kFastBlocksPerSM;
     const int grid = (int)(tiles < slots ? tiles : slots);
     cudaError_t e = cudaSuccess;
 #define AVB_LAUNCH_K(...)                                                                          \
@@ -304,19 +292,14 @@ inline int fast_launch(const FastParams& p, size_t smem, int sum_mode, cudaStrea
                                  cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);          \
         if (e == cudaSuccess) fast_pass_kernel<__VA_ARGS__><<<grid, kFastThreads, smem, st>>>(p);  \
     } while (0)
-#define AVB_LAUNCH_HV(...)                                                                         \
-    do {                                                                                           \
-        if (p.is_v) AVB_LAUNCH_K(__VA_ARGS__); else AVB_LAUNCH_K(__VA_ARGS__);                      \
-    } while (0)
     // chain-specialised instantiations (the BASELINE configs); anything else runs the
     // chain-generic instantiation
     const FastAxis& a = p.ax;
     const int v0 = a.s[0].variant, v1 = a.nsteps > 1 ? a.s[1].variant : -1,
               v2 = a.nsteps > 2 ? a.s[2].variant : -1;
     const int cs = p.rtaps_step;
-    const bool generic_only = false;
 #define AVB_TRY(SUMM, NSS, A0, A1, A2, CSS)                                                         \
-    if (!launched && !generic_only && sum_mode == SUMM && a.nsteps == NSS && v0 == A0 &&           \
+    if (!launched && sum_mode == SUMM && a.nsteps == NSS && v0 == A0 &&           \
         (NSS < 2 || v1 == A1) && (NSS < 3 || v2 == A2) && cs == CSS) {                             \
         if (p.is_v && plain_f32) AVB_LAUNCH_K(SUMM, true, NSS, A0, A1, A2, CSS, 1);                 \
         else if (p.is_v && int_plain) AVB_LAUNCH_K(SUMM, true, NSS, A0, A1, A2, CSS, 2);            \
@@ -343,7 +326,6 @@ inline int fast_launch(const FastParams& p, size_t smem, int sum_mode, cudaStrea
         }
     }
 #undef AVB_TRY
-#undef AVB_LAUNCH_HV
 #undef AVB_LAUNCH_K
     if (e != cudaSuccess) return -1;
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
@@ -390,8 +372,6 @@ inline const int* fast_tile_table(const FastPass& fp, int out0, int out1) {
     return d;
 }
 
-inline size_t fast_elsize(int t) { return t == AVIRB200_U8 ? 1 : (t == AVIRB200_U16 ? 2 : 4); }
-
 // Picks the (single) resize step whose one effective phase goes into the kernel parameters.
 inline void fast_set_const_taps(FastParams& p, const FastPass& fp) {
     p.debug = 0; // (the kernels' perf-experiment branches are never enabled from the library)
@@ -418,9 +398,10 @@ inline void fast_set_footprint(FastParams& p, const FastFootprint& f) {
 
 // Returns 0 = launched, -2 = not applicable (alignment: the caller runs the generic kernel),
 // -1 = launch error.
-inline int fast_row_pass(const FastPlan& f, const avirb200_plan_desc& d, const void* d_src,
-                         size_t src_pitch, float* d_mid, int rows, const float* lut, cudaStream_t st) {
-    const size_t es = fast_elsize(d.in_type);
+// mid_pitch: floats between intermediate rows.
+inline int fast_row_pass(const FastPlan& f, const avirb200_plan_desc& d, const void* d_src, size_t src_pitch,
+                         float* d_mid, size_t mid_pitch, int rows, const float* lut, int sm_count, cudaStream_t st) {
+    const size_t es = elem_size(d.in_type);
     if (((uintptr_t)d_src % (4 * es)) != 0 || (src_pitch % 4) != 0 || ((uintptr_t)d_mid % 16) != 0)
         return -2;
     FastParams p;
@@ -436,14 +417,14 @@ inline int fast_row_pass(const FastPlan& f, const avirb200_plan_desc& d, const v
     p.tile_ranges = fast_tile_table(f.h, 0, d.dst_w);
     if (p.tile_ranges == nullptr) return -1;
     p.src = d_src; p.src_pitch = (long long)src_pitch; p.src_type = d.in_type;
-    p.dst = d_mid; p.dst_pitch = (long long)d.dst_w * 4; p.dst_type = AVIRB200_F32;
-    return fast_launch(p, f.h.fpnt.smem, d.sum_mode, st);
+    p.dst = d_mid; p.dst_pitch = (long long)mid_pitch; p.dst_type = AVIRB200_F32;
+    return fast_launch(p, f.h.fpnt.smem, d.sum_mode, sm_count, st);
 }
 
-inline int fast_col_pass(const FastPlan& f, const avirb200_plan_desc& d, const float* d_mid,
+inline int fast_col_pass(const FastPlan& f, const avirb200_plan_desc& d, const float* d_mid, size_t mid_pitch,
                          int mid_row_base, void* d_dst, size_t dst_pitch, int out0, int out1,
-                         const float* lut, cudaStream_t st) {
-    const size_t es = fast_elsize(d.out_type);
+                         const float* lut, int sm_count, cudaStream_t st) {
+    const size_t es = elem_size(d.out_type);
     if (((uintptr_t)d_dst % (2 * es)) != 0 || (dst_pitch % 2) != 0 || ((uintptr_t)d_mid % 16) != 0)
         return -2;
     FastParams p;
@@ -463,11 +444,11 @@ inline int fast_col_pass(const FastPlan& f, const avirb200_plan_desc& d, const f
     fast_set_const_taps(p, f.v);
     p.tile_ranges = fast_tile_table(f.v, out0, out1);
     if (p.tile_ranges == nullptr) return -1;
-    p.src = d_mid; p.src_pitch = (long long)d.dst_w * 4; p.src_type = AVIRB200_F32;
+    p.src = d_mid; p.src_pitch = (long long)mid_pitch; p.src_type = AVIRB200_F32;
     p.src_row_base = mid_row_base;
     p.dst = d_dst; p.dst_pitch = (long long)dst_pitch; p.dst_type = d.out_type;
     p.dst_row_base = out0;
-    return fast_launch(p, fpnt.smem, d.sum_mode, st);
+    return fast_launch(p, fpnt.smem, d.sum_mode, sm_count, st);
 }
 
 } // namespace avb

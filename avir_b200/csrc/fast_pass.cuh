@@ -13,6 +13,7 @@
 #include <vector>
 
 #include "fast_kernel.cuh"
+#include "host_util.h"
 
 namespace avb {
 

@@ -28,23 +28,12 @@
 #include <vector>
 
 #include "avirb200.h"
+#include "host_util.h"
+
+using avb::elem_size;
+using avb::fail;
 
 namespace {
-
-thread_local std::string g_lerr;
-
-int lfail(int code, const std::string& m) {
-    g_lerr = m;
-    return code;
-}
-
-#define LCUDA_TRY(expr)                                                                    \
-    do {                                                                                   \
-        cudaError_t e_ = (expr);                                                           \
-        if (e_ != cudaSuccess)                                                             \
-            return lfail(e_ == cudaErrorMemoryAllocation ? AVIRB200_ERR_ALLOC : AVIRB200_ERR_CUDA, \
-                         std::string(#expr) + ": " + cudaGetErrorString(e_));              \
-    } while (0)
 
 struct LAxis {
     int src_len, dst_len, kl, nphases;
@@ -290,8 +279,6 @@ __global__ void __launch_bounds__(256) lancir_row4_kernel(const __grid_constant_
             make_ushort4((unsigned short)a, (unsigned short)b, (unsigned short)c, (unsigned short)d);
 }
 
-size_t lsize(int t) { return t == AVIRB200_U8 ? 1 : (t == AVIRB200_U16 ? 2 : 4); }
-
 } // namespace
 
 struct lancirb200_plan {
@@ -310,35 +297,34 @@ struct lancirb200_plan {
 extern "C" {
 
 int lancirb200_plan_create(const lancirb200_plan_desc* d, lancirb200_plan** out) {
-    if (d == nullptr || out == nullptr) return lfail(AVIRB200_ERR_BAD_ARG, "null argument");
+    if (d == nullptr || out == nullptr) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
     *out = nullptr;
-    if (d->channels < 1 || d->channels > 4) return lfail(AVIRB200_ERR_BAD_ARG, "channels must be 1..4");
+    if (d->channels < 1 || d->channels > 4) return fail(AVIRB200_ERR_BAD_ARG, "channels must be 1..4");
     if (d->v.kernel_len < 4 || d->h.kernel_len < 4 || ((d->v.kernel_len | d->h.kernel_len) & 1))
-        return lfail(AVIRB200_ERR_BAD_ARG, "kernel length must be even and >= 4");
+        return fail(AVIRB200_ERR_BAD_ARG, "kernel length must be even and >= 4");
     if (d->src_w < 1 || d->src_h < 1 || d->dst_w < 1 || d->dst_h < 1)
-        return lfail(AVIRB200_ERR_BAD_ARG, "bad geometry");
+        return fail(AVIRB200_ERR_BAD_ARG, "bad geometry");
     for (int a = 0; a < 2; ++a) {
         const lancirb200_axis_desc& ax = a ? d->h : d->v;
         if (ax.kernel_len < 2 || ax.nphases < 1 || !ax.taps || !ax.src_pos || !ax.phase)
-            return lfail(AVIRB200_ERR_BAD_ARG, "bad axis tables");
+            return fail(AVIRB200_ERR_BAD_ARG, "bad axis tables");
         for (int i = 0; i < ax.dst_len; ++i)
             if (ax.phase[i] < 0 || ax.phase[i] >= ax.nphases)
-                return lfail(AVIRB200_ERR_BAD_ARG, "phase index out of range");
+                return fail(AVIRB200_ERR_BAD_ARG, "phase index out of range");
     }
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
-        return lfail(AVIRB200_ERR_NO_DEVICE, "no CUDA device");
+        return fail(AVIRB200_ERR_NO_DEVICE, "no CUDA device");
     std::unique_ptr<lancirb200_plan> pl(new (std::nothrow) lancirb200_plan());
-    if (!pl) return lfail(AVIRB200_ERR_ALLOC, "host allocation failed");
+    if (!pl) return fail(AVIRB200_ERR_ALLOC, "host allocation failed");
     pl->desc = *d;
-    LCUDA_TRY(cudaGetDevice(&pl->device));
-    auto al = [](size_t v) { return (v + 255) / 256 * 256; };
+    CUDA_TRY(cudaGetDevice(&pl->device));
     size_t bytes = 0;
     for (int a = 0; a < 2; ++a) {
         const lancirb200_axis_desc& ax = a ? d->h : d->v;
-        bytes += al((size_t)ax.nphases * ax.kernel_len * 4) + 2 * al((size_t)ax.dst_len * 4);
+        bytes += avb::align_up((size_t)ax.nphases * ax.kernel_len * 4, 256) + 2 * avb::align_up((size_t)ax.dst_len * 4, 256);
     }
-    LCUDA_TRY(cudaMalloc(&pl->arena, bytes));
+    CUDA_TRY(cudaMalloc(&pl->arena, bytes));
     std::vector<char> img(bytes, 0);
     size_t off = 0;
     for (int a = 0; a < 2; ++a) {
@@ -349,14 +335,14 @@ int lancirb200_plan_create(const lancirb200_plan_desc* d, lancirb200_plan** out)
         char* base = static_cast<char*>(pl->arena);
         size_t n = (size_t)ax.nphases * ax.kernel_len * 4;
         std::memcpy(img.data() + off, ax.taps, n);
-        da.taps = reinterpret_cast<const float*>(base + off); off += al(n);
+        da.taps = reinterpret_cast<const float*>(base + off); off += avb::align_up(n, 256);
         n = (size_t)ax.dst_len * 4;
         std::memcpy(img.data() + off, ax.src_pos, n);
-        da.src_pos = reinterpret_cast<const int*>(base + off); off += al(n);
+        da.src_pos = reinterpret_cast<const int*>(base + off); off += avb::align_up(n, 256);
         std::memcpy(img.data() + off, ax.phase, n);
-        da.phase = reinterpret_cast<const int*>(base + off); off += al(n);
+        da.phase = reinterpret_cast<const int*>(base + off); off += avb::align_up(n, 256);
     }
-    LCUDA_TRY(cudaMemcpy(pl->arena, img.data(), bytes, cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(pl->arena, img.data(), bytes, cudaMemcpyHostToDevice));
     pl->desc.v.taps = nullptr; pl->desc.h.taps = nullptr;
     *out = pl.release();
     return 0;
@@ -370,14 +356,14 @@ void lancirb200_plan_destroy(lancirb200_plan* pl) {
 }
 
 int lancirb200_plan_workspace_bytes(const lancirb200_plan* pl, size_t* bytes) {
-    if (!pl || !bytes) return lfail(AVIRB200_ERR_BAD_ARG, "null argument");
+    if (!pl || !bytes) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
     *bytes = (size_t)pl->desc.dst_h * pl->desc.src_w * pl->desc.channels * sizeof(float);
     return 0;
 }
 
 int lancirb200_resize_device(const lancirb200_plan* pl, const void* d_src, size_t src_pitch,
                              void* d_dst, size_t dst_pitch, void* d_ws, void* stream) {
-    if (!pl || !d_src || !d_dst || !d_ws) return lfail(AVIRB200_ERR_BAD_ARG, "null argument");
+    if (!pl || !d_src || !d_dst || !d_ws) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
     const lancirb200_plan_desc& d = pl->desc;
     LParams p;
     p.v = pl->dv; p.h = pl->dh;
@@ -388,12 +374,12 @@ int lancirb200_resize_device(const lancirb200_plan* pl, const void* d_src, size_
     p.mid = static_cast<float*>(d_ws);
     p.dst = d_dst; p.dst_pitch = (long long)dst_pitch;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (d.dst_h > 65535) return lfail(AVIRB200_ERR_UNSUPPORTED, "image too tall");
+    if (d.dst_h > 65535) return fail(AVIRB200_ERR_UNSUPPORTED, "image too tall");
     (void)cudaGetLastError(); // (a stale non-sticky error of another library is not this launch's)
     // 4-channel images whose pixels are aligned to their own size: the vector kernels
-    const bool vec_in = d.channels == 4 && (src_pitch % 4) == 0 && ((uintptr_t)d_src % (4 * lsize(d.in_type))) == 0 &&
+    const bool vec_in = d.channels == 4 && (src_pitch % 4) == 0 && ((uintptr_t)d_src % (4 * elem_size(d.in_type))) == 0 &&
                         ((uintptr_t)d_ws % 16) == 0;
-    const bool vec_out = d.channels == 4 && (dst_pitch % 4) == 0 && ((uintptr_t)d_dst % (4 * lsize(d.out_type))) == 0 &&
+    const bool vec_out = d.channels == 4 && (dst_pitch % 4) == 0 && ((uintptr_t)d_dst % (4 * elem_size(d.out_type))) == 0 &&
                          ((uintptr_t)d_ws % 16) == 0;
     if (vec_in) {
         dim3 g1((d.src_w + 255) / 256, (d.dst_h + kLColRows - 1) / kLColRows);
@@ -435,41 +421,41 @@ int lancirb200_resize_device(const lancirb200_plan* pl, const void* d_src, size_
         dim3 g2((d.dst_w * d.channels + 255) / 256, d.dst_h);
         lancir_row_kernel<<<g2, 256, 0, st>>>(p);
     }
-    LCUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaGetLastError());
     return 0;
 }
 
 int lancirb200_resize_host(lancirb200_plan* pl, const void* h_src, size_t src_pitch, void* h_dst,
                            size_t dst_pitch) {
-    if (!pl || !h_src || !h_dst) return lfail(AVIRB200_ERR_BAD_ARG, "null argument");
+    if (!pl || !h_src || !h_dst) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
     const lancirb200_plan_desc& d = pl->desc;
     std::lock_guard<std::mutex> lk(pl->mx);
-    LCUDA_TRY(cudaSetDevice(pl->device));
-    const size_t in_row = (size_t)d.src_w * d.channels * lsize(d.in_type);
-    const size_t out_row = (size_t)d.dst_w * d.channels * lsize(d.out_type);
+    CUDA_TRY(cudaSetDevice(pl->device));
+    const size_t in_row = (size_t)d.src_w * d.channels * elem_size(d.in_type);
+    const size_t out_row = (size_t)d.dst_w * d.channels * elem_size(d.out_type);
     size_t ws = 0;
     lancirb200_plan_workspace_bytes(pl, &ws);
-    if (!pl->stream) LCUDA_TRY(cudaStreamCreateWithFlags(&pl->stream, cudaStreamNonBlocking));
+    if (!pl->stream) CUDA_TRY(cudaStreamCreateWithFlags(&pl->stream, cudaStreamNonBlocking));
     if (pl->src_bytes < in_row * d.src_h) {
         cudaFree(pl->d_src); pl->d_src = nullptr; pl->src_bytes = 0;
-        LCUDA_TRY(cudaMalloc(&pl->d_src, in_row * d.src_h)); pl->src_bytes = in_row * d.src_h;
+        CUDA_TRY(cudaMalloc(&pl->d_src, in_row * d.src_h)); pl->src_bytes = in_row * d.src_h;
     }
     if (pl->dst_bytes < out_row * d.dst_h) {
         cudaFree(pl->d_dst); pl->d_dst = nullptr; pl->dst_bytes = 0;
-        LCUDA_TRY(cudaMalloc(&pl->d_dst, out_row * d.dst_h)); pl->dst_bytes = out_row * d.dst_h;
+        CUDA_TRY(cudaMalloc(&pl->d_dst, out_row * d.dst_h)); pl->dst_bytes = out_row * d.dst_h;
     }
     if (pl->ws_bytes < ws) {
         cudaFree(pl->d_ws); pl->d_ws = nullptr; pl->ws_bytes = 0;
-        LCUDA_TRY(cudaMalloc(&pl->d_ws, ws)); pl->ws_bytes = ws;
+        CUDA_TRY(cudaMalloc(&pl->d_ws, ws)); pl->ws_bytes = ws;
     }
-    LCUDA_TRY(cudaMemcpy2DAsync(pl->d_src, in_row, h_src, src_pitch * lsize(d.in_type), in_row,
+    CUDA_TRY(cudaMemcpy2DAsync(pl->d_src, in_row, h_src, src_pitch * elem_size(d.in_type), in_row,
                                 d.src_h, cudaMemcpyHostToDevice, pl->stream));
     int r = lancirb200_resize_device(pl, pl->d_src, (size_t)d.src_w * d.channels, pl->d_dst,
                                      (size_t)d.dst_w * d.channels, pl->d_ws, pl->stream);
     if (r != 0) return r;
-    LCUDA_TRY(cudaMemcpy2DAsync(h_dst, dst_pitch * lsize(d.out_type), pl->d_dst, out_row, out_row,
+    CUDA_TRY(cudaMemcpy2DAsync(h_dst, dst_pitch * elem_size(d.out_type), pl->d_dst, out_row, out_row,
                                 d.dst_h, cudaMemcpyDeviceToHost, pl->stream));
-    LCUDA_TRY(cudaStreamSynchronize(pl->stream));
+    CUDA_TRY(cudaStreamSynchronize(pl->stream));
     return 0;
 }
 

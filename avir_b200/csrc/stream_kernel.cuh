@@ -57,7 +57,6 @@ using avb::lin2srgb;
 using avb::round_out;
 using avb::round_out_int;
 
-constexpr int kLines = 16;      // lines per warp (2 lanes per line)
 constexpr int kEpiXs = 4;       // row pass "epilogue" code: sender of the fused halo exchange (StreamParams xs_*)
 constexpr int kPitchL = 32;     // float2 units: [position][lane] rows of 256 bytes
 // Row pass, source ring and output staging: [line][position][4 channels] with one pixel of

@@ -13,6 +13,7 @@
 namespace avs {
 
 constexpr int kMaxSteps = 3;
+constexpr int kLines = 16; // lines per warp (2 lanes per line): the 16-line strips of a pass
 // Source code of the row pass beyond the plain element types: u8 pixels linearised on the way
 // in (sRGB table for the colour channels, (float) b * InGammaMult for alpha; avir.h:2843-2931).
 constexpr int kSrcU8Srgb = 4;
@@ -260,7 +261,7 @@ inline int stream_row_source_code(const avirb200_plan_desc& d) {
     return (d.use_gamma & 1) ? kSrcU8Srgb : d.in_type;
 }
 
-// Kernel parameters of one pass (the caller fills the image pointers / bases).
+// Kernel parameters of one pass without its buffers (stream_fill_row_params / _col_params add them).
 inline void stream_fill_params(StreamParams& p, const StreamAxisPlan& ap, const avirb200_plan_desc& d) {
     memset(&p, 0, sizeof p);
     for (int i = 0; i < ap.nsteps; ++i) p.s[i] = ap.s[i];
@@ -276,6 +277,120 @@ inline void stream_fill_params(StreamParams& p, const StreamAxisPlan& ap, const 
     p.tr_mul = d.tr_mul;
     p.tr_mul_inv = d.tr_mul_inv;
     p.pk_out = d.pk_out;
+}
+
+// Row pass: every output column of `rows` source rows from `src` into the intermediate rows at `mid`
+// (pitches in elements).  seg_top / seg_bot: only the first seg_top and the last seg_bot of those rows,
+// in one launch (seg_bot > 0: two line segments).
+inline void stream_fill_row_params(StreamParams& p, const StreamAxisPlan& ap, const avirb200_plan_desc& d,
+                                   const void* src, long long src_pitch, float* mid, long long mid_pitch, int rows,
+                                   const float* lut, int seg_top = 0, int seg_bot = 0) {
+    stream_fill_params(p, ap, d);
+    p.n_lines = rows;
+    if (seg_bot > 0) {
+        p.seg_a = seg_top;
+        p.seg_b = seg_bot;
+        p.seg_b_line0 = rows - seg_bot;
+    } else if (seg_top > 0) {
+        p.n_lines = seg_top;
+    }
+    p.out0 = 0;
+    p.out1 = d.dst_w;
+    p.src = src;
+    p.src_type = stream_row_source_code(d);
+    p.srgb_lut = lut;
+    p.src_pitch = src_pitch;
+    p.dst = mid;
+    p.dst_pitch = mid_pitch;
+    p.dst_type = AVIRB200_F32;
+}
+
+// Column pass: destination rows [out0, out1) into `dst` (its row 0 = row out0) from the intermediate rows
+// [mid_lo, mid_hi) the buffer at `mid` holds (its row 0 = row mid_lo).
+inline void stream_fill_col_params(StreamParams& p, const StreamAxisPlan& ap, const avirb200_plan_desc& d,
+                                   const float* mid, long long mid_pitch, int mid_lo, int mid_hi, void* dst,
+                                   long long dst_pitch, int out0, int out1) {
+    stream_fill_params(p, ap, d);
+    p.n_lines = d.dst_w;
+    p.out0 = out0;
+    p.out1 = out1;
+    p.src = mid;
+    p.src_pitch = mid_pitch;
+    p.src_row_base = mid_lo;
+    p.src_lo = mid_lo;
+    p.src_hi = mid_hi;
+    p.dst = dst;
+    p.dst_pitch = dst_pitch;
+    p.dst_type = d.out_type;
+    p.dst_row_base = out0;
+}
+
+// ---- fused halo exchange of sharded calls (StreamParams xs_* / xr_*) --------------------------------
+// A band's mailbox as the kernels see it: the rows received from the band above and from the band below,
+// the two flags (flags[0]: the rows from above are in, flags[1]: the rows from below) and the two
+// counters the band's own row pass keeps as sender (count[0]: rows going up, count[1]: down).
+struct StreamMailbox {
+    float* from_up = nullptr;
+    float* from_dn = nullptr;
+    unsigned* flags = nullptr;
+    unsigned long long* count = nullptr;
+};
+
+// One band of a sharded call and its neighbours (up / dn: null at the ends of the image), with the
+// mailboxes of all three for the call's sequence number.  The band sends its first up->halo_down rows
+// to the band above and its last dn->halo_up rows to the band below.
+struct StreamLink {
+    const avirb200_shard_info* me = nullptr;
+    const avirb200_shard_info* up = nullptr;
+    const avirb200_shard_info* dn = nullptr;
+    StreamMailbox mine, above, below;
+    unsigned seq = 0;
+};
+inline int stream_rows_up(const StreamLink& l) { return l.up ? l.up->halo_down : 0; }
+inline int stream_rows_down(const StreamLink& l) { return l.dn ? l.dn->halo_up : 0; }
+
+// The fused halves run only between neighbours that exchange rows in BOTH directions.  Slots alternate
+// per call and are reused two calls later; what orders the reuse is that a band's call n+1 needs its
+// neighbour's call-n+1 rows, which the neighbour sends after its call-n column pass.
+inline bool stream_fused_rx_ok(const StreamLink& l) {
+    return (l.up == nullptr || (stream_rows_up(l) > 0) == (l.me->halo_up > 0)) &&
+           (l.dn == nullptr || (stream_rows_down(l) > 0) == (l.me->halo_down > 0));
+}
+// The fused sender counts per direction over whole 16-line strips: not for a band so short that one
+// strip holds rows of both neighbours.
+inline bool stream_fused_tx_ok(const StreamLink& l) {
+    const int top = stream_rows_up(l), bot = stream_rows_down(l);
+    return stream_fused_rx_ok(l) && !(top > 0 && bot > 0 && (top + kLines - 1) / kLines > (l.me->src_rows - bot) / kLines);
+}
+
+// Row pass as sender: the band's boundary rows also go into the neighbours' mailboxes.
+inline void stream_set_sender(StreamParams& p, const StreamLink& l) {
+    const int top = stream_rows_up(l), bot = stream_rows_down(l), rows = l.me->src_rows;
+    p.xs_seq = l.seq;
+    p.xs_count = l.mine.count;
+    if (top > 0) {
+        p.xs_up_dst = l.above.from_dn;
+        p.xs_up_flag = &l.above.flags[1];
+        p.xs_top = top;
+        p.xs_units[0] = (unsigned long long)((top + kLines - 1) / kLines);
+    }
+    if (bot > 0) {
+        p.xs_dn_dst = l.below.from_up;
+        p.xs_dn_flag = &l.below.flags[0];
+        p.xs_bot0 = rows - bot;
+        p.xs_bot = bot;
+        p.xs_units[1] = (unsigned long long)((rows + kLines - 1) / kLines - p.xs_bot0 / kLines);
+    }
+}
+
+// Column pass as receiver: the neighbours' rows are read in place from the band's own mailbox.
+inline void stream_set_receiver(StreamParams& p, const StreamLink& l) {
+    p.xr_up_src = l.mine.from_up;
+    p.xr_dn_src = l.mine.from_dn;
+    p.xr_flags = l.mine.flags;
+    p.xr_seq = l.seq;
+    p.xr_own_lo = l.me->src_row0;
+    p.xr_own_hi = l.me->src_row0 + l.me->src_rows;
 }
 
 } // namespace avs

@@ -39,9 +39,11 @@ static const unsigned char* g_hi = nullptr;
 static const unsigned char* g_alt_lo[2] = {nullptr, nullptr};
 static const unsigned char* g_alt_hi[2] = {nullptr, nullptr};
 
+#include "host_util.h"
 #include "stream_kernel.cuh"
 
 using namespace avs;
+using avb::elem_size;
 
 namespace {
 
@@ -112,68 +114,45 @@ int stream_emul_resize(const avirb200_plan_desc* d, const void* src, size_t src_
     if (!stream_row_source_ok(*d) || !stream_plan_axis(d->h, d->sum_mode, d->channels, h, allow) ||
         !stream_plan_axis(d->v, d->sum_mode, d->channels, v, allow))
         return -4;
-    std::vector<float> mid((size_t)d->src_h * d->dst_w * 4);
+    const size_t rowf = (size_t)d->dst_w * 4, in_es = elem_size(d->in_type), out_es = elem_size(d->out_type);
+    std::vector<float> mid((size_t)d->src_h * rowf);
     StreamParams p;
-    stream_fill_params(p, h, *d);
-    p.n_lines = d->src_h;
-    p.out0 = 0;
-    p.out1 = d->dst_w;
-    p.src = src;
-    p.src_type = stream_row_source_code(*d);
-    p.srgb_lut = lut;
-    p.src_pitch = (long long)src_pitch;
-    p.dst = mid.data();
-    p.dst_pitch = (long long)d->dst_w * 4;
-    p.dst_type = AVIRB200_F32;
     g_oob = 0;
-    {
-        const size_t esz = (d->in_type == AVIRB200_U8) ? 1 : (d->in_type == AVIRB200_U16 ? 2 : 4);
-        g_lo = static_cast<const unsigned char*>(src);
-        g_hi = g_lo + ((size_t)(d->src_h - 1) * src_pitch + (size_t)d->src_w * 4) * esz;
-    }
+    g_lo = static_cast<const unsigned char*>(src);
+    g_hi = g_lo + ((size_t)(d->src_h - 1) * src_pitch + (size_t)d->src_w * 4) * in_es;
     if (seg_top + seg_bot > 0 && seg_top + seg_bot < d->src_h) {
         // as a sharded call schedules the row pass: the first seg_top and last seg_bot rows in one
         // segmented launch, then the rows between
-        StreamParams q = p;
-        if (seg_bot > 0) { q.seg_a = seg_top; q.seg_b = seg_bot; q.seg_b_line0 = d->src_h - seg_bot; }
-        else q.n_lines = seg_top;
-        if (!emul_dispatch<false>(h.chain, variant, q, warps_h, 0)) return -4;
-        const size_t esz = (d->in_type == AVIRB200_U8) ? 1 : (d->in_type == AVIRB200_U16 ? 2 : 4);
-        q = p;
-        q.n_lines = d->src_h - seg_top - seg_bot;
-        q.src = static_cast<const unsigned char*>(src) + (size_t)seg_top * src_pitch * esz;
-        q.dst = mid.data() + (size_t)seg_top * d->dst_w * 4;
-        if (!emul_dispatch<false>(h.chain, variant, q, warps_h, 0)) return -4;
-    } else if (!emul_dispatch<false>(h.chain, variant, p, warps_h, 0)) return -4;
+        stream_fill_row_params(p, h, *d, src, (long long)src_pitch, mid.data(), (long long)rowf, d->src_h, lut, seg_top,
+                               seg_bot);
+        if (!emul_dispatch<false>(h.chain, variant, p, warps_h, 0)) return -4;
+        stream_fill_row_params(p, h, *d, static_cast<const unsigned char*>(src) + (size_t)seg_top * src_pitch * in_es,
+                               (long long)src_pitch, mid.data() + (size_t)seg_top * rowf, (long long)rowf,
+                               d->src_h - seg_top - seg_bot, lut);
+        if (!emul_dispatch<false>(h.chain, variant, p, warps_h, 0)) return -4;
+    } else {
+        stream_fill_row_params(p, h, *d, src, (long long)src_pitch, mid.data(), (long long)rowf, d->src_h, lut);
+        if (!emul_dispatch<false>(h.chain, variant, p, warps_h, 0)) return -4;
+    }
 
     const int epi = stream_epilogue_code(*d);
     for (int b = 0; b < bands; ++b) {
-        stream_fill_params(p, v, *d);
-        p.n_lines = d->dst_w;
-        p.out0 = (int)((long long)d->dst_h * b / bands);
-        p.out1 = (int)((long long)d->dst_h * (b + 1) / bands);
-        if (p.out1 <= p.out0) continue;
-        p.src = mid.data();
-        p.src_pitch = (long long)d->dst_w * 4;
-        p.src_row_base = 0;
-        g_lo = reinterpret_cast<const unsigned char*>(mid.data());
-        g_hi = g_lo + mid.size() * sizeof(float);
+        const int out0 = (int)((long long)d->dst_h * b / bands), out1 = (int)((long long)d->dst_h * (b + 1) / bands);
+        if (out1 <= out0) continue;
+        const float* msrc = mid.data();
+        int lo = 0, hi = d->src_h;
         std::vector<float> bandbuf;
         if (need != nullptr) { // the band's own rows only, as on a rank of the sharded schedule
-            const int r0 = need[2 * b], nr = need[2 * b + 1];
-            const size_t rowf = (size_t)d->dst_w * 4;
-            bandbuf.assign(mid.begin() + (size_t)r0 * rowf, mid.begin() + (size_t)(r0 + nr) * rowf);
-            p.src = bandbuf.data();
-            p.src_row_base = r0;
-            p.src_lo = r0;
-            p.src_hi = r0 + nr;
-            g_lo = reinterpret_cast<const unsigned char*>(bandbuf.data());
-            g_hi = g_lo + bandbuf.size() * sizeof(float);
+            lo = need[2 * b];
+            hi = lo + need[2 * b + 1];
+            bandbuf.assign(mid.begin() + (size_t)lo * rowf, mid.begin() + (size_t)hi * rowf);
+            msrc = bandbuf.data();
         }
-        p.dst = dst;
-        p.dst_pitch = (long long)dst_pitch;
-        p.dst_type = d->out_type;
-        p.dst_row_base = 0;
+        g_lo = reinterpret_cast<const unsigned char*>(msrc);
+        g_hi = g_lo + (size_t)(hi - lo) * rowf * sizeof(float);
+        stream_fill_col_params(p, v, *d, msrc, (long long)rowf, lo, hi,
+                               static_cast<unsigned char*>(dst) + (size_t)out0 * dst_pitch * out_es, (long long)dst_pitch,
+                               out0, out1);
         if (!emul_dispatch<true>(v.chain, variant, p, warps_v, epi)) return -4;
     }
     g_lo = g_hi = nullptr;
@@ -186,8 +165,9 @@ int stream_emul_resize(const avirb200_plan_desc* d, const void* src, size_t src_
 // reads its own rows from its buffer and the neighbours' rows in place from its mailbox.
 // info: avirb200_shard_info of every band (8 ints each).  Every buffer is NaN-poisoned and exactly as
 // large as the rows it is meant to hold; reads are bounds-checked (-5), flags and counters are
-// checked after the row passes (-6).  Returns 1, nothing computed, where the product would not run the
-// fused sender (a band so short that one 16-line strip holds rows of both neighbours).
+// checked after the row passes (-6).  The parameters and the eligibility rule are the engine's own
+// (stream_types.h: stream_set_sender / _receiver, stream_fused_tx_ok).  Returns 1, nothing computed,
+// where the product would not run the fused sender for some band.
 int stream_emul_resize_fused(const avirb200_plan_desc* d, const void* src, size_t src_pitch, void* dst,
                              size_t dst_pitch, int warps_h, int warps_v, int bands, int variant, const float* lut,
                              int allow, const int* info) {
@@ -196,85 +176,58 @@ int stream_emul_resize_fused(const avirb200_plan_desc* d, const void* src, size_
         !stream_plan_axis(d->v, d->sum_mode, d->channels, v, allow))
         return -4;
     struct Band {
-        int src_row0, src_rows, dst_row0, dst_rows, need_row0, need_rows, halo_up, halo_down;
+        avirb200_shard_info si;
         std::vector<float> own, box_up, box_dn; // box_up: rows from the band above, box_dn: from the band below
         unsigned flags[2] = {0, 0};
         unsigned long long count[2] = {0, 0};
+        StreamLink link;
     };
-    const size_t rowf = (size_t)d->dst_w * 4;
+    const size_t rowf = (size_t)d->dst_w * 4, in_es = elem_size(d->in_type), out_es = elem_size(d->out_type);
     const float nanv = __builtin_nanf("");
+    const unsigned seq = 5;
     std::vector<Band> B(bands);
     for (int b = 0; b < bands; ++b) {
-        const int* q = info + 8 * b;
         Band& x = B[b];
-        x.src_row0 = q[0]; x.src_rows = q[1]; x.dst_row0 = q[2]; x.dst_rows = q[3];
-        x.need_row0 = q[4]; x.need_rows = q[5]; x.halo_up = q[6]; x.halo_down = q[7];
-        x.own.assign((size_t)x.src_rows * rowf, nanv);
-        x.box_up.assign((size_t)x.halo_up * rowf, nanv);
-        x.box_dn.assign((size_t)x.halo_down * rowf, nanv);
+        memcpy(&x.si, info + 8 * b, sizeof x.si);
+        x.own.assign((size_t)x.si.src_rows * rowf, nanv);
+        x.box_up.assign((size_t)x.si.halo_up * rowf, nanv);
+        x.box_dn.assign((size_t)x.si.halo_down * rowf, nanv);
+        x.link.me = &x.si;
+        x.link.mine = {x.box_up.data(), x.box_dn.data(), x.flags, x.count};
+        x.link.seq = seq;
     }
-    const size_t esz = (d->in_type == AVIRB200_U8) ? 1 : (d->in_type == AVIRB200_U16 ? 2 : 4);
-    const unsigned seq = 5;
+    for (int b = 0; b < bands; ++b) {
+        StreamLink& l = B[b].link;
+        if (b > 0) { l.up = &B[b - 1].si; l.above = B[b - 1].link.mine; }
+        if (b + 1 < bands) { l.dn = &B[b + 1].si; l.below = B[b + 1].link.mine; }
+        if (stream_rows_up(l) > B[b].si.src_rows || stream_rows_down(l) > B[b].si.src_rows) return -4;
+        if (!stream_fused_tx_ok(l)) return 1; // the product runs the copy-engine exchange
+    }
     g_oob = 0;
     g_alt_lo[0] = g_alt_lo[1] = g_alt_hi[0] = g_alt_hi[1] = nullptr;
     StreamParams p;
     for (int b = 0; b < bands; ++b) {
         Band& x = B[b];
-        stream_fill_params(p, h, *d);
-        p.n_lines = x.src_rows;
-        p.out0 = 0;
-        p.out1 = d->dst_w;
-        p.src = static_cast<const unsigned char*>(src) + (size_t)x.src_row0 * src_pitch * esz;
-        p.src_type = stream_row_source_code(*d);
-        p.srgb_lut = lut;
-        p.src_pitch = (long long)src_pitch;
-        p.dst = x.own.data();
-        p.dst_pitch = (long long)d->dst_w * 4;
-        p.dst_type = AVIRB200_F32;
-        g_lo = static_cast<const unsigned char*>(p.src);
-        g_hi = g_lo + ((size_t)(x.src_rows - 1) * src_pitch + (size_t)d->src_w * 4) * esz;
-        const int top = (b > 0) ? B[b - 1].halo_down : 0, bot = (b + 1 < bands) ? B[b + 1].halo_up : 0;
-        if (top > x.src_rows || bot > x.src_rows) return -4;
-        if (top > 0 && bot > 0 && (top + kLines - 1) / kLines > (x.src_rows - bot) / kLines) return 1; // a strip with rows of both neighbours: the product pushes
-        p.xs_seq = seq;
-        p.xs_count = x.count;
-        if (top > 0) {
-            p.xs_up_dst = B[b - 1].box_dn.data();
-            p.xs_up_flag = &B[b - 1].flags[1];
-            p.xs_top = top;
-            p.xs_units[0] = (unsigned long long)((top + kLines - 1) / kLines);
-        }
-        if (bot > 0) {
-            p.xs_dn_dst = B[b + 1].box_up.data();
-            p.xs_dn_flag = &B[b + 1].flags[0];
-            p.xs_bot0 = x.src_rows - bot;
-            p.xs_bot = bot;
-            p.xs_units[1] = (unsigned long long)((x.src_rows + kLines - 1) / kLines - p.xs_bot0 / kLines);
-        }
+        const unsigned char* bsrc = static_cast<const unsigned char*>(src) + (size_t)x.si.src_row0 * src_pitch * in_es;
+        stream_fill_row_params(p, h, *d, bsrc, (long long)src_pitch, x.own.data(), (long long)rowf, x.si.src_rows, lut);
+        stream_set_sender(p, x.link);
+        g_lo = bsrc;
+        g_hi = g_lo + ((size_t)(x.si.src_rows - 1) * src_pitch + (size_t)d->src_w * 4) * in_es;
         if (!emul_dispatch<false>(h.chain, variant, p, warps_h, 0)) return -4;
         if (x.count[0] != 0 || x.count[1] != 0) return -6;
-        if (top > 0 && B[b - 1].flags[1] != seq) return -6;
-        if (bot > 0 && B[b + 1].flags[0] != seq) return -6;
+        if (stream_rows_up(x.link) > 0 && B[b - 1].flags[1] != seq) return -6;
+        if (stream_rows_down(x.link) > 0 && B[b + 1].flags[0] != seq) return -6;
     }
     const int epi = stream_epilogue_code(*d);
     for (int b = 0; b < bands; ++b) {
         Band& x = B[b];
-        if (x.dst_rows <= 0) continue;
-        stream_fill_params(p, v, *d);
-        p.n_lines = d->dst_w;
-        p.out0 = x.dst_row0;
-        p.out1 = x.dst_row0 + x.dst_rows;
-        p.src = x.own.data() - (ptrdiff_t)x.halo_up * (ptrdiff_t)rowf; // (row need_row0 of a buffer that only holds the own rows)
-        p.src_pitch = (long long)d->dst_w * 4;
-        p.src_row_base = x.need_row0;
-        p.src_lo = x.need_row0;
-        p.src_hi = x.need_row0 + x.need_rows;
-        p.xr_up_src = x.box_up.data();
-        p.xr_dn_src = x.box_dn.data();
-        p.xr_flags = x.flags;
-        p.xr_seq = seq;
-        p.xr_own_lo = x.src_row0;
-        p.xr_own_hi = x.src_row0 + x.src_rows;
+        if (x.si.dst_rows <= 0) continue;
+        // (row need_row0 of a buffer that only holds the own rows)
+        stream_fill_col_params(p, v, *d, x.own.data() - (ptrdiff_t)x.si.halo_up * (ptrdiff_t)rowf, (long long)rowf,
+                               x.si.need_row0, x.si.need_row0 + x.si.need_rows,
+                               static_cast<unsigned char*>(dst) + (size_t)x.si.dst_row0 * dst_pitch * out_es,
+                               (long long)dst_pitch, x.si.dst_row0, x.si.dst_row0 + x.si.dst_rows);
+        stream_set_receiver(p, x.link);
         g_lo = reinterpret_cast<const unsigned char*>(x.own.data());
         g_hi = g_lo + x.own.size() * sizeof(float);
         g_alt_lo[0] = reinterpret_cast<const unsigned char*>(x.box_up.data());
@@ -283,10 +236,6 @@ int stream_emul_resize_fused(const avirb200_plan_desc* d, const void* src, size_
         g_alt_hi[1] = g_alt_lo[1] + x.box_dn.size() * sizeof(float);
         if (x.box_up.empty()) g_alt_lo[0] = g_alt_hi[0] = nullptr;
         if (x.box_dn.empty()) g_alt_lo[1] = g_alt_hi[1] = nullptr;
-        p.dst = dst;
-        p.dst_pitch = (long long)dst_pitch;
-        p.dst_type = d->out_type;
-        p.dst_row_base = 0;
         if (!emul_dispatch<true>(v.chain, variant, p, warps_v, epi)) return -4;
     }
     g_lo = g_hi = nullptr;

@@ -44,6 +44,28 @@ def test_bad_arguments_are_rejected_before_touching_cuda():
     assert lib.avirb200_shard_query_desc(None, 0, 1, info) == -1
 
 
+class _LancirAxis(C.Structure):
+    _fields_ = [("src_len", C.c_int32), ("dst_len", C.c_int32), ("kernel_len", C.c_int32), ("nphases", C.c_int32),
+                ("taps", C.c_void_p), ("src_pos", C.c_void_p), ("phase", C.c_void_p)]
+
+
+class _LancirDesc(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("src_w", "src_h", "dst_w", "dst_h", "channels", "in_type", "out_type")] + [
+        ("out_mul", C.c_float), ("is_unity_mul", C.c_int32), ("clamp_max", C.c_float),
+        ("v", _LancirAxis), ("h", _LancirAxis)]
+
+
+def test_lancir_failures_are_reported_by_last_error():
+    """avirb200_last_error() reports a LANCIR failure with LANCIR's own message, not an older one."""
+    lib = ab.lib()
+    out = C.c_void_p()
+    assert lib.avirb200_plan_create(None, C.byref(out)) == -1
+    assert lib.avirb200_last_error() == b"null argument"
+    desc = _LancirDesc(src_w=8, src_h=8, dst_w=4, dst_h=4, channels=5)
+    assert lib.lancirb200_plan_create(C.byref(desc), C.byref(out)) == -1
+    assert lib.avirb200_last_error() == b"channels must be 1..4"
+
+
 @pytest.mark.skipif(ab.device_count() > 0, reason="checks the no-GPU behaviour")
 def test_no_cpu_fallback_without_gpu():
     """Without a device the product must fail loudly, never compute on the host."""

@@ -74,6 +74,9 @@ def host_lib():
                                                                                     C.c_void_p]
         h.avirb200_host_workspace_bytes.restype = C.c_longlong
         h.avirb200_host_workspace_bytes.argtypes = call + geom
+        h.avirb200_host_window.restype = C.c_int
+        h.avirb200_host_window.argtypes = ([C.c_int] + h.avirb200_host_resize.argtypes + [C.c_int] * 4 +
+                                           [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p])
         h.lancirb200_host_resize.restype = C.c_int
         h.lancirb200_host_resize.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int,
                                              C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
@@ -174,6 +177,46 @@ class CImageResizer:
             NewWidth, NewHeight, ch, k, ox, oy, g, a, bm, d_workspace, stream)
         if r != 0:
             raise AvirB200Error(host_lib().avirb200_host_last_error().decode())
+
+    def _window(self, op, src, src_shape, in_dtype, src_pitch, dst, NewWidth, NewHeight, out_dtype, k, aVars,
+                window, d_workspace=None, stream=0):
+        sh, sw, ch = src_shape
+        ox, oy, g, a, bm = self._vars(aVars)
+        info, nbytes = (C.c_int * 6)(), C.c_longlong(0)
+        r = host_lib().avirb200_host_window(op, *self._call(_T[np.dtype(in_dtype)], _T[np.dtype(out_dtype)]), src, sw,
+                                            sh, src_pitch, dst, NewWidth, NewHeight, ch, k, ox, oy, g, a, bm,
+                                            *window, d_workspace, stream, info, C.byref(nbytes))
+        if r != 0:
+            raise AvirB200Error(host_lib().avirb200_host_last_error().decode())
+        return list(info), nbytes.value
+
+    def resizeImageWindow(self, SrcBuf, NewWidth, NewHeight, window, k=0.0, aVars=None, out_dtype=None,
+                          NewBuf=None, SrcScanlineSize=0):
+        """The destination window (x0, y0, w, h) of resizeImage(SrcBuf, NewWidth, NewHeight, ...):
+        SrcBuf is the whole source (host), the result is an (h, w, C) array (GPU extension)."""
+        src = _scanlines(SrcBuf, SrcScanlineSize, "resizeImageWindow")
+        out_dtype = np.dtype(out_dtype or src.dtype)
+        dst = NewBuf if NewBuf is not None else np.empty((window[3], window[2], src.shape[2]), out_dtype)
+        self._window(0, src.ctypes.data, src.shape, src.dtype, SrcScanlineSize, dst.ctypes.data, NewWidth,
+                     NewHeight, out_dtype, k, aVars, window)
+        return dst
+
+    def resizeImageWindowDevice(self, d_src, src_shape, in_dtype, d_dst, NewWidth, NewHeight, out_dtype, window,
+                                d_workspace, k=0.0, aVars=None, stream=0, SrcScanlineSize=0):
+        """Device pointers: d_src at the window's footprint (windowFootprint), d_dst receives the (h, w, C)
+        window; src_shape is the WHOLE source's (H, W, C).  Asynchronous on `stream`."""
+        self._window(1, d_src, src_shape, in_dtype, SrcScanlineSize, d_dst, NewWidth, NewHeight, out_dtype, k, aVars,
+                     window, d_workspace, stream)
+
+    def windowFootprint(self, src_shape, in_dtype, NewWidth, NewHeight, out_dtype, window, k=0.0, aVars=None):
+        """dict of avirb200_window_info: the source columns / rows the window reads."""
+        info, _ = self._window(2, None, src_shape, in_dtype, 0, None, NewWidth, NewHeight, out_dtype, k, aVars,
+                               window)
+        return dict(zip(("src_x0", "src_w", "src_y0", "src_h", "mid_row0", "mid_rows"), info))
+
+    def windowWorkspaceBytes(self, src_shape, in_dtype, NewWidth, NewHeight, out_dtype, window, k=0.0, aVars=None):
+        return self._window(3, None, src_shape, in_dtype, 0, None, NewWidth, NewHeight, out_dtype, k, aVars,
+                            window)[1]
 
     def descriptor(self, src_shape, in_dtype, NewWidth, NewHeight, out_dtype, k=0.0, aVars=None):
         """Host-only: the C-ABI plan descriptor resizeImage would hand to the GPU library.

@@ -152,12 +152,13 @@ def build_emul(force=False):
         return _build_emul(force)
 
 
-def _build_emul(force=False):
-    """TEST INFRASTRUCTURE: host lockstep emulation of the streaming kernel (tests/emul)."""
+def _build_emul(force=False, name="stream_emul"):
+    """TEST INFRASTRUCTURE: host lockstep emulation of the streaming kernel (tests/emul): lib<name>.so
+    from <name>.cpp (window_emul.cpp: the windowed passes, on stream_emul.cpp's emulation)."""
     d = os.path.join(ROOT, "tests", "emul")
-    target = os.path.join(d, "libstream_emul.so")
-    src = os.path.join(d, "stream_emul.cpp")
-    deps = [src] + _sources([CSRC, INC], (".cuh", ".h"))
+    target = os.path.join(d, "lib%s.so" % name)
+    src = os.path.join(d, name + ".cpp")
+    deps = [src, os.path.join(d, "stream_emul.cpp")] + _sources([CSRC, INC], (".cuh", ".h"))
     if not force and not _newer(target, deps):
         return target
     cuda_inc = os.path.join(os.path.dirname(os.path.dirname(_nvcc())), "include")
@@ -168,11 +169,17 @@ def _build_emul(force=False):
     return target
 
 
+def build_window_emul(force=False):
+    with _BuildLock():
+        return _build_emul(force, "window_emul")
+
+
 def build_all(force=False, verbose=False):
     build_cuda(force, verbose)
     build_host(force)
     build_oracles()
     build_emul(force)
+    build_window_emul(force)
 
 
 if __name__ == "__main__":

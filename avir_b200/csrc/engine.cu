@@ -326,8 +326,11 @@ int launch_narrow(int type, const void* src, void* dst, size_t dst_pitch, int w,
 // 1..3-channel plans whose passes run on the 4-channel kernels in this call (avirb200_plan::pad4)
 bool use_pad4(const avirb200_plan* pl) { return pl->pad4 && pl->opt_family != 1; }
 
-// Floats between consecutive intermediate rows, for every kernel family and every band / halo offset.
-size_t mid_pitch(const avirb200_plan* pl) { return (size_t)pl->desc.dst_w * pl->mid_ch; }
+// Floats between consecutive intermediate rows, for every kernel family and every band / halo offset
+// (cols: the intermediate columns a window's passes run over; < 0: the whole destination width).
+size_t mid_pitch(const avirb200_plan* pl, int cols = -1) {
+    return (size_t)(cols >= 0 ? cols : pl->desc.dst_w) * pl->mid_ch;
+}
 
 // Whether a pass runs on the streaming kernel with these buffers (the kernel's source / destination as
 // it sees them: a widened plan's scratch copies).  The copies move whole pixels: the row pass's source
@@ -349,34 +352,40 @@ bool col_pass_on_stream(const avirb200_plan* pl, const void* dst, size_t dst_pit
 // band's first seg_top and last seg_bot rows, in ONE launch.
 // xs (sharded calls, fused halo exchange): the band's link, sent through the streaming kernel; *xs_done
 // tells whether the streaming kernel took the pass (and so delivered the neighbours' rows).
+// cols (windows): only the intermediate columns [out0, out1), stored from d_mid's column 0 on, from a
+// source buffer whose column 0 is source column src_lo and that holds columns [src_lo, src_hi); null:
+// every column of the whole source line.
 int run_row_pass(const avirb200_plan* pl, const void* d_src, size_t src_pitch, float* d_mid,
                  int rows, cudaStream_t st, int* launches, void* scratch4 = nullptr, int seg_top = 0, int seg_bot = 0,
-                 const avs::StreamLink* xs = nullptr, bool* xs_done = nullptr) {
+                 const avs::StreamLink* xs = nullptr, bool* xs_done = nullptr, const avs::StreamColumns* cols = nullptr) {
     if (rows <= 0) return 0;
     // (a non-sticky error another library left in this thread -- NCCL's peer-access probing leaves
     // cudaErrorPeerAccessAlreadyEnabled once the IPC mailboxes have enabled it -- is not this launch's)
     (void)cudaGetLastError();
     const avirb200_plan_desc& d = pl->desc;
+    const avs::StreamColumns cr = cols ? *cols : avs::StreamColumns{0, d.dst_w, 0, d.src_w};
+    const size_t mp = mid_pitch(pl, cr.out1 - cr.out0);
     const bool p4 = use_pad4(pl);
     if (p4) {
         if (scratch4 == nullptr) return fail(AVIRB200_ERR_BAD_ARG, "row pass: no scratch for the widened source");
-        if (launch_widen(d.in_type, d_src, src_pitch, scratch4, d.src_w, rows, d.channels, st) != 0)
+        if (launch_widen(d.in_type, d_src, src_pitch, scratch4, cr.src_hi - cr.src_lo, rows, d.channels, st) != 0)
             return fail(AVIRB200_ERR_CUDA, "widening the source failed");
         ++*launches;
         d_src = scratch4;
-        src_pitch = (size_t)d.src_w * 4;
+        src_pitch = (size_t)(cr.src_hi - cr.src_lo) * 4;
     }
     if (row_pass_on_stream(pl, d_src, src_pitch, d_mid)) {
         avs::StreamParams sp;
-        avs::stream_fill_row_params(sp, pl->stream_h, d, d_src, (long long)src_pitch, d_mid, (long long)mid_pitch(pl), rows,
-                                    pl->d_lut, seg_top, seg_bot);
+        avs::stream_fill_row_params(sp, pl->stream_h, d, d_src, (long long)src_pitch, d_mid, (long long)mp, rows,
+                                    pl->d_lut, seg_top, seg_bot, cols);
         if (xs != nullptr) avs::stream_set_sender(sp, *xs);
         const int r = avs::stream_launch(pl->stream_h.chain, false, 0, pl->opt_var_h, sp, pl->sm_count, st);
         if (r == -1) return fail(AVIRB200_ERR_CUDA, "streaming row pass launch failed");
         if (r == 0) { ++*launches; if (xs_done) *xs_done = (xs != nullptr); return 0; }
     }
     if (pl->opt_family != 1 && pl->fast.h_ok) {
-        const int r = fast_row_pass(pl->fast, d, d_src, src_pitch, d_mid, mid_pitch(pl), rows, pl->d_lut, pl->sm_count, st);
+        const int r = fast_row_pass(pl->fast, d, d_src, src_pitch, d_mid, mp, rows, pl->d_lut, pl->sm_count, st,
+                                    cr.out0, cr.out1, cr.src_lo);
         if (r == -1) return fail(AVIRB200_ERR_CUDA, "fast row pass launch failed");
         if (r == 0) { ++*launches; return 0; }
     }
@@ -385,23 +394,26 @@ int run_row_pass(const avirb200_plan* pl, const void* d_src, size_t src_pitch, f
     PassParams p;
     std::memset(&p, 0, sizeof p);
     fill_common(p, pl);
-    const PassConfig c = p4 ? choose_generic_config(pl->h.hostdev, 4, 0, d.dst_w) : pl->cfg_h;
+    const PassConfig c = (p4 || cols != nullptr) ? choose_generic_config(pl->h.hostdev, p4 ? 4 : d.channels, cr.out0, cr.out1)
+                                                 : pl->cfg_h;
     if (p4) p.channels = 4;
     p.ax = pl->h.dev;
     p.is_v = 0;
     p.n_lines = rows;
     p.lines_per_block = c.lines_per_block;
     p.tile_out = c.tile_out;
-    p.out0 = 0;
-    p.out1 = d.dst_w;
+    p.out0 = cr.out0;
+    p.out1 = cr.out1;
     p.span = c.span;
     p.pitch = c.pitch;
     p.src = d_src;
     p.src_pitch = (long long)src_pitch;
     p.src_type = d.in_type;
+    p.src_row_base = cr.src_lo;
     p.dst = d_mid;
-    p.dst_pitch = (long long)mid_pitch(pl);
+    p.dst_pitch = (long long)mp;
     p.dst_type = AVIRB200_F32;
+    p.dst_row_base = cr.out0;
     ++*launches;
     return launch_generic(p, c, st);
 }
@@ -411,12 +423,15 @@ int run_row_pass(const avirb200_plan* pl, const void* d_src, size_t src_pitch, f
 // xr (sharded calls, fused halo exchange): the band's link -- the neighbours' rows are read in place from
 // its mailbox.  Returns 1, nothing launched, when the streaming kernel cannot take the pass (the caller
 // moves the rows into the workspace and calls again without xr).
+// cols (windows): pixel columns of the intermediate and the destination (< 0: the destination width).
 int run_col_pass(const avirb200_plan* pl, const float* d_mid, int mid_row_base, void* d_dst,
                  size_t dst_pitch, int out0, int out1, cudaStream_t st, int* launches, void* scratch4 = nullptr,
-                 int mid_rows = -1, const avs::StreamLink* xr = nullptr) {
+                 int mid_rows = -1, const avs::StreamLink* xr = nullptr, int cols = -1) {
     if (out1 <= out0) return 0;
     (void)cudaGetLastError(); // (see run_row_pass)
-    const avirb200_plan_desc& d = pl->desc;
+    // (a window's column pass is the whole image's on a narrower intermediate: dst_w = its columns)
+    avirb200_plan_desc d = pl->desc;
+    if (cols >= 0) d.dst_w = cols;
     const bool p4 = use_pad4(pl);
     void* const user_dst = d_dst;
     const size_t user_pitch = dst_pitch;
@@ -434,7 +449,7 @@ int run_col_pass(const avirb200_plan* pl, const float* d_mid, int mid_row_base, 
     };
     if (col_pass_on_stream(pl, d_dst, dst_pitch, d_mid)) {
         avs::StreamParams sp;
-        avs::stream_fill_col_params(sp, pl->stream_v, d, d_mid, (long long)mid_pitch(pl), mid_row_base,
+        avs::stream_fill_col_params(sp, pl->stream_v, d, d_mid, (long long)mid_pitch(pl, d.dst_w), mid_row_base,
                                     (mid_rows >= 0) ? mid_row_base + mid_rows : d.src_h, d_dst, (long long)dst_pitch,
                                     out0, out1);
         if (xr != nullptr) avs::stream_set_receiver(sp, *xr);
@@ -445,7 +460,7 @@ int run_col_pass(const avirb200_plan* pl, const float* d_mid, int mid_row_base, 
     }
     if (xr != nullptr) return 1;
     if (pl->opt_family != 1 && pl->fast.v_ok) {
-        const int r = fast_col_pass(pl->fast, d, d_mid, mid_pitch(pl), mid_row_base, d_dst, dst_pitch, out0, out1,
+        const int r = fast_col_pass(pl->fast, d, d_mid, mid_pitch(pl, d.dst_w), mid_row_base, d_dst, dst_pitch, out0, out1,
                                     pl->d_lut, pl->sm_count, st);
         if (r == -1) return fail(AVIRB200_ERR_CUDA, "fast column pass launch failed");
         if (r == 0) { ++*launches; return finish(); }
@@ -469,7 +484,7 @@ int run_col_pass(const avirb200_plan* pl, const float* d_mid, int mid_row_base, 
     p.span = c.span;
     p.pitch = c.pitch;
     p.src = d_mid;
-    p.src_pitch = (long long)mid_pitch(pl);
+    p.src_pitch = (long long)mid_pitch(pl, d.dst_w);
     p.src_type = AVIRB200_F32;
     p.src_row_base = mid_row_base;
     p.dst = d_dst;
@@ -564,6 +579,32 @@ int shard_compute_axis(const DevAxis& vaxis, int rank, int nranks, avirb200_shar
 
 int shard_compute(const avirb200_plan* pl, int rank, int nranks, avirb200_shard_info* info) {
     return shard_compute_axis(pl->v.hostdev, rank, nranks, info);
+}
+
+// A destination window's footprint: the source columns / rows both chains read for it.  errd: the plan
+// diffuses the rounding error (a window of it is not a window of the whole image's result).
+int window_compute(const DevAxis& h, const DevAxis& v, bool errd, int x0, int y0, int w, int hh,
+                   avirb200_window_info* info) {
+    if (w < 1 || hh < 1 || x0 < 0 || y0 < 0 || (long long)x0 + w > h.dst_len || (long long)y0 + hh > v.dst_len)
+        return fail(AVIRB200_ERR_BAD_ARG, "window empty or outside the destination");
+    if (errd) return fail(AVIRB200_ERR_UNSUPPORTED, "windows: error diffusion depends on every pixel before the window");
+    const Range cx = chain_source_range(h, Range{x0, x0 + w - 1}, nullptr);
+    const Range cy = chain_source_range(v, Range{y0, y0 + hh - 1}, nullptr);
+    info->src_x0 = cx.a;
+    info->src_w = cx.b - cx.a + 1;
+    info->src_y0 = info->mid_row0 = cy.a;
+    info->src_h = info->mid_rows = cy.b - cy.a + 1;
+    return 0;
+}
+
+int window_compute(const avirb200_plan* pl, int x0, int y0, int w, int h, avirb200_window_info* info) {
+    const int r = window_compute(pl->h.hostdev, pl->v.hostdev, pl->errd, x0, y0, w, h, info);
+    // (the tile kernel's tables of the window's column and row ranges: built now, not inside a launch)
+    if (r == 0) {
+        fast_prepare_columns(pl->fast, x0, x0 + w);
+        fast_prepare_range(pl->fast, y0, y0 + h);
+    }
+    return r;
 }
 
 // ---- error-diffusion ditherer (upstream CImageResizerDithererErrdINL / ErrdDIL) ---------------
@@ -756,43 +797,53 @@ __global__ void __launch_bounds__(256) widen_f32_kernel(const float* __restrict_
 int errd_groups(const avirb200_plan* pl) { return (pl->desc.dst_h + 31) / 32; }
 
 // The workspace of one call: byte offsets of its segments, in this order, each 256-byte aligned.
-//   mid        the intermediate: mid_rows rows of mid_pitch() floats (at offset 0)
-//   in32       float copy of a double source                                  } whole-image calls only
-//   out32      float copy of the destination (double output, error diffusion) } (resize_device):
-//   errd_bnd   error diffusion: boundary rows, one per 32-row group           } sharded and per-pass
-//   errd_prog  error diffusion: progress counters                             } calls refuse such plans
-//   src4       the widened source of src_rows rows   } widened plans (pad4) only
-//   dst4       the widened destination of dst_rows rows }
+// A call covers src_rows x src_cols source pixels, mid_rows x dst_cols intermediate pixels and
+// dst_rows x dst_cols destination pixels (the whole image, a shard's band or a window and its footprint).
+//   mid        the intermediate: mid_rows rows of mid_pitch(dst_cols) floats (at offset 0)
+//   in32       float copy of a double source                                  } whole-image and window
+//   out32      float copy of the destination (double output, error diffusion) } calls only: sharded
+//   errd_bnd   error diffusion: boundary rows, one per 32-row group           } and per-pass calls refuse
+//   errd_prog  error diffusion: progress counters                             } such plans (windows: errd)
+//   src4       the widened source      } widened plans (pad4) only
+//   dst4       the widened destination }
 // Segments a plan does not use are empty.
 struct WsLayout {
     size_t in32, out32, errd_bnd, errd_prog, src4, dst4, total;
 };
-WsLayout ws_layout(const avirb200_plan* pl, int mid_rows, int src_rows, int dst_rows, bool whole) {
+WsLayout ws_layout(const avirb200_plan* pl, int mid_rows, int src_rows, int dst_rows, bool whole, int src_cols,
+                   int dst_cols) {
     const avirb200_plan_desc& d = pl->desc;
     const bool f64_in = whole && pl->io_in_type == AVIRB200_F64;
     const bool f32_out = whole && (pl->io_out_type == AVIRB200_F64 || pl->errd);
     const bool errd = whole && pl->errd;
     WsLayout w;
-    size_t off = align_up((size_t)mid_rows * mid_pitch(pl) * sizeof(float), 256);
+    size_t off = align_up((size_t)mid_rows * mid_pitch(pl, dst_cols) * sizeof(float), 256);
     auto seg = [&](bool on, size_t bytes) {
         const size_t at = off;
         if (on) off += align_up(bytes, 256);
         return at;
     };
-    w.in32 = seg(f64_in, (size_t)d.src_w * d.src_h * d.channels * sizeof(float));
-    w.out32 = seg(f32_out, (size_t)d.dst_w * d.dst_h * d.channels * sizeof(float));
+    w.in32 = seg(f64_in, (size_t)src_cols * src_rows * d.channels * sizeof(float));
+    w.out32 = seg(f32_out, (size_t)dst_cols * dst_rows * d.channels * sizeof(float));
     w.errd_bnd = seg(errd, (size_t)errd_groups(pl) * d.dst_w * d.channels * sizeof(float));
     w.errd_prog = seg(errd, (size_t)errd_groups(pl) * sizeof(int));
-    w.src4 = seg(pl->pad4, (size_t)src_rows * d.src_w * 4 * elem_size(d.in_type));
-    w.dst4 = seg(pl->pad4, (size_t)dst_rows * d.dst_w * 4 * elem_size(d.out_type));
+    w.src4 = seg(pl->pad4, (size_t)src_rows * src_cols * 4 * elem_size(d.in_type));
+    w.dst4 = seg(pl->pad4, (size_t)dst_rows * dst_cols * 4 * elem_size(d.out_type));
     w.total = off;
     return w;
 }
 // The whole image's layout (resize_device, the per-pass entry points, the banded host call).
-WsLayout ws_layout(const avirb200_plan* pl) { return ws_layout(pl, pl->desc.src_h, pl->desc.src_h, pl->desc.dst_h, true); }
+WsLayout ws_layout(const avirb200_plan* pl) {
+    const avirb200_plan_desc& d = pl->desc;
+    return ws_layout(pl, d.src_h, d.src_h, d.dst_h, true, d.src_w, d.dst_w);
+}
 // One band of the sharded schedule.
 WsLayout ws_layout(const avirb200_plan* pl, const avirb200_shard_info& si) {
-    return ws_layout(pl, si.need_rows, si.src_rows, si.dst_rows, false);
+    return ws_layout(pl, si.need_rows, si.src_rows, si.dst_rows, false, pl->desc.src_w, pl->desc.dst_w);
+}
+// A destination window of w columns and h rows with its footprint wi.
+WsLayout ws_layout(const avirb200_plan* pl, const avirb200_window_info& wi, int w, int h) {
+    return ws_layout(pl, wi.mid_rows, wi.src_h, h, true, wi.src_w, w);
 }
 
 // ---- host-call staging: one set of device buffers per device, shared by every plan ----------------
@@ -1358,12 +1409,17 @@ int avirb200_plan_workspace_bytes(const avirb200_plan* pl, size_t* bytes) {
 
 int avirb200_plan_last_launches(const avirb200_plan* pl) { return pl ? pl->last_launches : 0; }
 
-int avirb200_resize_device(const avirb200_plan* pl, const void* d_src, size_t src_pitch, void* d_dst,
-                           size_t dst_pitch, void* d_ws, void* stream) {
-    if (pl == nullptr || d_src == nullptr || d_dst == nullptr || d_ws == nullptr)
-        return fail(AVIRB200_ERR_BAD_ARG, "null argument");
+} // extern "C"
+
+namespace {
+
+// The whole image (win null), or the destination window [x0, x0 + w) x [y0, y0 + h) with its footprint
+// *win: d_src holds the footprint, d_dst receives the window.
+int resize_region(const avirb200_plan* pl, const avirb200_window_info* win, int x0, int y0, int w, int h,
+                  const void* d_src, size_t src_pitch, void* d_dst, size_t dst_pitch, void* d_ws, void* stream) {
     const avirb200_plan_desc& d = pl->desc;
-    if (src_pitch < (size_t)d.src_w * d.channels || dst_pitch < (size_t)d.dst_w * d.channels)
+    const int src_w = win ? win->src_w : d.src_w, src_h = win ? win->src_h : d.src_h;
+    if (src_pitch < (size_t)src_w * d.channels || dst_pitch < (size_t)w * d.channels)
         return fail(AVIRB200_ERR_BAD_ARG, "pitch smaller than a row");
     {
         int cur = -1;
@@ -1373,7 +1429,7 @@ int avirb200_resize_device(const avirb200_plan* pl, const void* d_src, size_t sr
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     int launches = 0;
     char* wsb = static_cast<char*>(d_ws);
-    const WsLayout ws = ws_layout(pl);
+    const WsLayout ws = win ? ws_layout(pl, *win, w, h) : ws_layout(pl);
     float* in32 = reinterpret_cast<float*>(wsb + ws.in32);
     float* out32 = reinterpret_cast<float*>(wsb + ws.out32);
     const void* ksrc = d_src;
@@ -1381,27 +1437,37 @@ int avirb200_resize_device(const avirb200_plan* pl, const void* d_src, size_t sr
     void* kdst = d_dst;
     size_t kdst_pitch = dst_pitch;
     if (pl->io_in_type == AVIRB200_F64) {
-        const int re = d.src_w * d.channels;
-        const long long n = (long long)re * d.src_h;
+        const int re = src_w * d.channels;
+        const long long n = (long long)re * src_h;
         narrow_f64_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(static_cast<const double*>(d_src),
-                                                                       (long long)src_pitch, in32, re, d.src_h);
+                                                                       (long long)src_pitch, in32, re, src_h);
         ++launches;
         ksrc = in32;
         ksrc_pitch = (size_t)re;
     }
     if (pl->io_out_type == AVIRB200_F64 || pl->errd) {
         kdst = out32;
-        kdst_pitch = (size_t)d.dst_w * d.channels;
+        kdst_pitch = (size_t)w * d.channels;
     }
-    int r = run_row_pass(pl, ksrc, ksrc_pitch, static_cast<float*>(d_ws), d.src_h, st, &launches, wsb + ws.src4);
-    if (r != 0) return r;
-    r = run_col_pass(pl, static_cast<const float*>(d_ws), 0, kdst, kdst_pitch, 0, d.dst_h, st,
-                     &launches, wsb + ws.dst4);
+    int r;
+    if (win == nullptr) {
+        r = run_row_pass(pl, ksrc, ksrc_pitch, static_cast<float*>(d_ws), d.src_h, st, &launches, wsb + ws.src4);
+        if (r != 0) return r;
+        r = run_col_pass(pl, static_cast<const float*>(d_ws), 0, kdst, kdst_pitch, 0, d.dst_h, st,
+                         &launches, wsb + ws.dst4);
+    } else {
+        const avs::StreamColumns cols{x0, x0 + w, win->src_x0, win->src_x0 + win->src_w};
+        r = run_row_pass(pl, ksrc, ksrc_pitch, static_cast<float*>(d_ws), src_h, st, &launches, wsb + ws.src4, 0, 0,
+                         nullptr, nullptr, &cols);
+        if (r != 0) return r;
+        r = run_col_pass(pl, static_cast<const float*>(d_ws), win->mid_row0, kdst, kdst_pitch, y0, y0 + h, st,
+                         &launches, wsb + ws.dst4, win->mid_rows, nullptr, w);
+    }
     if (r == 0 && pl->io_out_type == AVIRB200_F64) {
-        const int re = d.dst_w * d.channels;
-        const long long n = (long long)re * d.dst_h;
+        const int re = w * d.channels;
+        const long long n = (long long)re * h;
         widen_f32_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(out32, static_cast<double*>(d_dst),
-                                                                      (long long)dst_pitch, re, d.dst_h);
+                                                                      (long long)dst_pitch, re, h);
         ++launches;
         CUDA_TRY(cudaGetLastError());
     }
@@ -1429,6 +1495,96 @@ int avirb200_resize_device(const avirb200_plan* pl, const void* d_src, size_t sr
     }
     pl->last_launches = launches;
     return r;
+}
+
+} // namespace
+
+extern "C" {
+
+int avirb200_resize_device(const avirb200_plan* pl, const void* d_src, size_t src_pitch, void* d_dst,
+                           size_t dst_pitch, void* d_ws, void* stream) {
+    if (pl == nullptr || d_src == nullptr || d_dst == nullptr || d_ws == nullptr)
+        return fail(AVIRB200_ERR_BAD_ARG, "null argument");
+    return resize_region(pl, nullptr, 0, 0, pl->desc.dst_w, pl->desc.dst_h, d_src, src_pitch, d_dst, dst_pitch, d_ws,
+                         stream);
+}
+
+int avirb200_window_query(const avirb200_plan* pl, int x0, int y0, int w, int h, avirb200_window_info* info) {
+    if (pl == nullptr || info == nullptr) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
+    return window_compute(pl, x0, y0, w, h, info);
+}
+
+int avirb200_window_query_desc(const avirb200_plan_desc* desc, int x0, int y0, int w, int h,
+                               avirb200_window_info* info) {
+    if (desc == nullptr || info == nullptr) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
+    if (desc->h.nsteps < 1 || desc->h.nsteps > AVIRB200_MAX_STEPS || desc->v.nsteps < 1 ||
+        desc->v.nsteps > AVIRB200_MAX_STEPS)
+        return fail(AVIRB200_ERR_BAD_ARG, "axis: nsteps out of range");
+    // (as avirb200_plan_create decides it)
+    const bool errd = desc->dither == 1 && (desc->out_type == AVIRB200_U8 || desc->out_type == AVIRB200_U16);
+    return window_compute(host_axis_view(desc->h), host_axis_view(desc->v), errd, x0, y0, w, h, info);
+}
+
+int avirb200_window_workspace_bytes(const avirb200_plan* pl, int x0, int y0, int w, int h, size_t* bytes) {
+    if (pl == nullptr || bytes == nullptr) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
+    avirb200_window_info wi;
+    const int r = window_compute(pl, x0, y0, w, h, &wi);
+    if (r != 0) return r;
+    *bytes = ws_layout(pl, wi, w, h).total;
+    return 0;
+}
+
+int avirb200_resize_window_device(const avirb200_plan* pl, int x0, int y0, int w, int h, const void* d_src,
+                                  size_t src_pitch, void* d_dst, size_t dst_pitch, void* d_ws, void* stream) {
+    if (pl == nullptr || d_src == nullptr || d_dst == nullptr || d_ws == nullptr)
+        return fail(AVIRB200_ERR_BAD_ARG, "null argument");
+    avirb200_window_info wi;
+    const int r = window_compute(pl->h.hostdev, pl->v.hostdev, pl->errd, x0, y0, w, h, &wi);
+    if (r != 0) return r;
+    return resize_region(pl, &wi, x0, y0, w, h, d_src, src_pitch, d_dst, dst_pitch, d_ws, stream);
+}
+
+int avirb200_resize_window_host(avirb200_plan* pl, int x0, int y0, int w, int h, const void* h_src,
+                                size_t src_pitch, void* h_dst, size_t dst_pitch) {
+    if (pl == nullptr || h_src == nullptr || h_dst == nullptr) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
+    const avirb200_plan_desc& d = pl->desc;
+    if (src_pitch < (size_t)d.src_w * d.channels || dst_pitch < (size_t)w * d.channels)
+        return fail(AVIRB200_ERR_BAD_ARG, "pitch smaller than a row");
+    avirb200_window_info wi;
+    int r = window_compute(pl->h.hostdev, pl->v.hostdev, pl->errd, x0, y0, w, h, &wi);
+    if (r != 0) return r;
+    std::lock_guard<std::mutex> lk(pl->mx);
+    // the call runs on the plan's device; the caller's current device is restored on every exit
+    struct DeviceGuard {
+        int prev = -1;
+        ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
+    } guard;
+    {
+        int cur = -1;
+        CUDA_TRY(cudaGetDevice(&cur));
+        if (cur != pl->device) {
+            CUDA_TRY(cudaSetDevice(pl->device));
+            guard.prev = cur;
+        }
+    }
+    size_t ws = 0;
+    if ((r = avirb200_window_workspace_bytes(pl, x0, y0, w, h, &ws)) != 0) return r;
+    std::lock_guard<std::mutex> sl(staging_of(pl->device).mx);
+    const size_t in_el = elem_size(pl->io_in_type), out_el = elem_size(pl->io_out_type);
+    const size_t in_row = (size_t)wi.src_w * d.channels * in_el, out_row = (size_t)w * d.channels * out_el;
+    if (pl->stream == nullptr) CUDA_TRY(cudaStreamCreateWithFlags(&pl->stream, cudaStreamNonBlocking));
+    if ((r = plan_staging(pl, in_row * wi.src_h, out_row * h, ws)) != 0) return r;
+    // the footprint only; the whole source is read before any destination pixel is written (aliasing)
+    const char* fsrc = static_cast<const char*>(h_src) + ((size_t)wi.src_y0 * src_pitch + (size_t)wi.src_x0 * d.channels) * in_el;
+    CUDA_TRY(cudaMemcpy2DAsync(pl->d_src, in_row, fsrc, src_pitch * in_el, in_row, wi.src_h, cudaMemcpyHostToDevice,
+                               pl->stream));
+    r = resize_region(pl, &wi, x0, y0, w, h, pl->d_src, (size_t)wi.src_w * d.channels, pl->d_dst, (size_t)w * d.channels,
+                      pl->d_ws, pl->stream);
+    if (r != 0) return r;
+    CUDA_TRY(cudaMemcpy2DAsync(h_dst, dst_pitch * out_el, pl->d_dst, out_row, out_row, h, cudaMemcpyDeviceToHost,
+                               pl->stream));
+    CUDA_TRY(cudaStreamSynchronize(pl->stream));
+    return 0;
 }
 
 int avirb200_row_pass_device(const avirb200_plan* pl, const void* d_src, size_t src_pitch,

@@ -227,6 +227,10 @@ inline const int* fast_tile_table(const FastPass& fp, int out0, int out1);
 inline void fast_prepare_range(const FastPlan& f, int out0, int out1) {
     if (f.v_ok && out1 > out0) fast_tile_table(f.v, out0, out1);
 }
+// The same for the row pass's intermediate columns [out0, out1) (windows).
+inline void fast_prepare_columns(const FastPlan& f, int out0, int out1) {
+    if (f.h_ok && out1 > out0) fast_tile_table(f.h, out0, out1);
+}
 
 inline void fast_plan_init(FastPlan& f, const DevAxis& h_host, const DevAxis& v_host,
                            const avirb200_plan_desc& d) {
@@ -399,26 +403,37 @@ inline void fast_set_footprint(FastParams& p, const FastFootprint& f) {
 // Returns 0 = launched, -2 = not applicable (alignment: the caller runs the generic kernel),
 // -1 = launch error.
 // mid_pitch: floats between intermediate rows.
+// A window: intermediate columns [out0, out1) (stored from the intermediate's column 0 on) from a source
+// buffer whose column 0 is source column src_col0; out1 < 0: every column of the whole line.
 inline int fast_row_pass(const FastPlan& f, const avirb200_plan_desc& d, const void* d_src, size_t src_pitch,
-                         float* d_mid, size_t mid_pitch, int rows, const float* lut, int sm_count, cudaStream_t st) {
+                         float* d_mid, size_t mid_pitch, int rows, const float* lut, int sm_count, cudaStream_t st,
+                         int out0 = 0, int out1 = -1, int src_col0 = 0) {
     const size_t es = elem_size(d.in_type);
     if (((uintptr_t)d_src % (4 * es)) != 0 || (src_pitch % 4) != 0 || ((uintptr_t)d_mid % 16) != 0)
         return -2;
+    if (out1 < 0) out1 = d.dst_w;
     FastParams p;
     memset(&p, 0, sizeof p);
     fast_fill_common(p, d, lut);
     p.ax = f.h.ax;
     p.is_v = 0;
     p.n_lines = rows;
+    FastFootprint fpnt = f.h.fpnt;
+    if (out0 != 0 || out1 != d.dst_w) { // a window: footprint of its own tiles
+        fpnt = fast_footprint_all(f.h.hax, f.h.tile_out, out0, out1, f.h.raw);
+        if (fpnt.smem > kFastSmemBudget) return -2;
+    }
     p.tile_out = f.h.tile_out;
-    p.out0 = 0; p.out1 = d.dst_w;
-    fast_set_footprint(p, f.h.fpnt);
+    p.out0 = out0; p.out1 = out1;
+    fast_set_footprint(p, fpnt);
     fast_set_const_taps(p, f.h);
-    p.tile_ranges = fast_tile_table(f.h, 0, d.dst_w);
+    p.tile_ranges = fast_tile_table(f.h, out0, out1);
     if (p.tile_ranges == nullptr) return -1;
     p.src = d_src; p.src_pitch = (long long)src_pitch; p.src_type = d.in_type;
+    p.src_row_base = src_col0;
     p.dst = d_mid; p.dst_pitch = (long long)mid_pitch; p.dst_type = AVIRB200_F32;
-    return fast_launch(p, f.h.fpnt.smem, d.sum_mode, sm_count, st);
+    p.dst_row_base = out0;
+    return fast_launch(p, fpnt.smem, d.sum_mode, sm_count, st);
 }
 
 inline int fast_col_pass(const FastPlan& f, const avirb200_plan_desc& d, const float* d_mid, size_t mid_pitch,

@@ -90,11 +90,11 @@ struct FastParams {
     const void* src;
     long long src_pitch;  // elements
     int src_type;
-    int src_row_base;
+    int src_row_base;     // source position held by the buffer's position 0 (column pass: row; row pass: column)
     void* dst;
     long long dst_pitch;
     int dst_type;
-    int dst_row_base;
+    int dst_row_base;     // final output stored at the destination's position 0 (column pass: row; row pass: column)
     int gamma_in, gamma_out, alpha_index;
     float in_gamma_mult, out_gamma_mult;
     const float* srgb_lut;
@@ -576,7 +576,7 @@ __device__ __forceinline__ void stage_source(const FastParams& p, float2* buf, c
     for (int r = r0; r < kFastLines; r += kFastThreads / 32) {
         const size_t rowoff = (size_t)(line0 + imin(r, nlines - 1)) * p.src_pitch;
         if (p.src_type == AVIRB200_F32) {
-            const float4* srow = reinterpret_cast<const float4*>(static_cast<const float*>(p.src) + rowoff);
+            const float4* srow = reinterpret_cast<const float4*>(static_cast<const float*>(p.src) + rowoff) - p.src_row_base;
             float2* d = buf + px * kFastPitch + r * 2;
             if (a >= 0 && a + n <= p.ax.src_len) {
                 const float4* g = srow + a + px; // interior tile: constant strides
@@ -594,7 +594,7 @@ __device__ __forceinline__ void stage_source(const FastParams& p, float2* buf, c
             }
         } else {
             for (int pos = px; pos < n; pos += 32) {
-                const int x = imin(imax(a + pos, 0), p.ax.src_len - 1);
+                const int x = imin(imax(a + pos, 0), p.ax.src_len - 1) - p.src_row_base;
                 float4 v;
                 if (p.src_type == AVIRB200_U8) {
                     const uchar4 b = __ldg(reinterpret_cast<const uchar4*>(static_cast<const unsigned char*>(p.src) + rowoff) + x);
@@ -641,7 +641,7 @@ __device__ __forceinline__ void stage_raw(const FastParams& p, unsigned char* ra
         const unsigned char* srow = static_cast<const unsigned char*>(p.src) +
                                     (size_t)(line0 + imin(r, nlines - 1)) * p.src_pitch * (pb / 4);
         for (int pos = px; pos < n; pos += 32) {
-            const int x = imin(imax(a + pos, 0), p.ax.src_len - 1);
+            const int x = imin(imax(a + pos, 0), p.ax.src_len - 1) - p.src_row_base;
             unsigned char* d = raw + ((size_t)pos * kFastLines + r) * pb;
             if (pb == 4) cp_async_small<4>(d, srow + (size_t)x * 4);
             else cp_async_small<8>(d, srow + (size_t)x * 8);
@@ -844,7 +844,7 @@ fast_pass_kernel(const __grid_constant__ FastParams p) {
             const int px = tid & 31, r0 = tid >> 5;
             for (int r = r0; r < nlines; r += kFastThreads / 32) {
                 float4* drow = reinterpret_cast<float4*>(static_cast<float*>(p.dst) +
-                                                         (size_t)(line0 + r) * p.dst_pitch);
+                                                         (size_t)(line0 + r) * p.dst_pitch) - p.dst_row_base;
                 for (int pos = px; pos < on; pos += 32)
                     drow[ro.a + pos] = *reinterpret_cast<const float4*>(ob + pos * kFastPitch + r * 2);
             }

@@ -34,19 +34,19 @@ struct PassParams {
     int n_lines;    // lines in this launch (rows for H, columns for V)
     int lines_per_block;
     int tile_out;   // final outputs per tile
-    int out0, out1; // final outputs [out0, out1) to produce (column pass on a shard)
+    int out0, out1; // final outputs [out0, out1) to produce (column pass on a shard, either pass of a window)
     int span;       // shared rows per buffer
     int pitch;      // shared row pitch in floats (odd)
     // source image / intermediate
     const void* src;
     long long src_pitch;  // elements between consecutive rows
     int src_type;         // avirb200_dtype (column pass: always F32)
-    int src_row_base;     // column pass: global row index of src row 0 (shards)
+    int src_row_base;     // global position of the buffer's position 0 (column pass: row; row pass: column)
     // destination
     void* dst;
     long long dst_pitch;
     int dst_type;
-    int dst_row_base;     // column pass: global dst row stored at dst row 0
+    int dst_row_base;     // global output stored at the destination's position 0 (column pass: row; row pass: column)
     // prologue / epilogue
     int gamma_in, gamma_out, alpha_index;
     float in_gamma_mult, out_gamma_mult;
@@ -245,7 +245,7 @@ generic_pass_kernel(const __grid_constant__ PassParams p) {
             for (int idx = threadIdx.x; idx < nlines * rowlen; idx += blockDim.x) {
                 const int r = idx / rowlen, e = idx - r * rowlen;
                 const int pos = e / C, c = e - pos * C;
-                const long long g = (long long)(line0 + r) * p.src_pitch + (long long)(a + pos) * C + c;
+                const long long g = (long long)(line0 + r) * p.src_pitch + (long long)(a + pos - p.src_row_base) * C + c;
                 b0[pos * p.pitch + r * C + c] = load_source(p, g, c);
             }
         }
@@ -289,7 +289,7 @@ generic_pass_kernel(const __grid_constant__ PassParams p) {
         for (int idx = threadIdx.x; idx < nlines * rowlen; idx += blockDim.x) {
             const int r = idx / rowlen, e = idx - r * rowlen;
             const int pos = e / C, c = e - pos * C;
-            const long long g = (long long)(line0 + r) * p.dst_pitch + (long long)(oa + pos) * C + c;
+            const long long g = (long long)(line0 + r) * p.dst_pitch + (long long)(oa + pos - p.dst_row_base) * C + c;
             ((float*)p.dst)[g] = ob[pos * p.pitch + r * C + c];
         }
     }

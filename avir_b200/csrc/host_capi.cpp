@@ -52,7 +52,7 @@ avir::CImageResizer<fpclass>& resizer_for(const CallArgs& a) {
     return *it->second;
 }
 
-enum Op { kDesc, kHost, kDevice, kWorkspace };
+enum Op { kDesc, kHost, kDevice, kWorkspace, kWinHost, kWinDevice, kWinFootprint, kWinWorkspace };
 
 struct OpArgs {
     Op op;
@@ -60,6 +60,8 @@ struct OpArgs {
     std::shared_ptr<avir::b200_detail::PlanHolder> holder;
     size_t bytes;
     int mode_h, mode_v;
+    int wx, wy, ww, wh;          // window ops: the destination window
+    avirb200_window_info info;   // kWinFootprint
 };
 
 template <class fpclass, class Tin, class Tout>
@@ -80,6 +82,18 @@ void run3(const CallArgs& a, OpArgs& o) {
         else if (o.op == kDevice)
             rs.resizeImageDevice((const Tin*)o.src, a.sw, a.sh, (int)o.src_pitch, (Tout*)o.dst,
                                  a.nw, a.nh, a.ch, a.k, o.workspace, &v);
+        else if (o.op == kWinHost)
+            rs.resizeImageWindow((const Tin*)o.src, a.sw, a.sh, (int)o.src_pitch, (Tout*)o.dst, a.nw, a.nh, a.ch,
+                                 a.k, o.wx, o.wy, o.ww, o.wh, &v);
+        else if (o.op == kWinDevice)
+            rs.resizeImageWindowDevice((const Tin*)o.src, a.sw, a.sh, (int)o.src_pitch, (Tout*)o.dst, a.nw, a.nh,
+                                       a.ch, a.k, o.wx, o.wy, o.ww, o.wh, o.workspace, &v);
+        else if (o.op == kWinFootprint)
+            o.info = rs.template windowFootprint<Tin, Tout>(a.sw, a.sh, a.nw, a.nh, a.ch, a.k, o.wx, o.wy, o.ww,
+                                                             o.wh, &v);
+        else if (o.op == kWinWorkspace)
+            o.bytes = rs.template windowWorkspaceBytes<Tin, Tout>(a.sw, a.sh, a.nw, a.nh, a.ch, a.k, o.wx, o.wy,
+                                                                   o.ww, o.wh, &v);
         else
             o.bytes = rs.template workspaceBytes<Tin, Tout>(a.sw, a.sh, a.nw, a.nh, a.ch, a.k, &v);
     }
@@ -353,6 +367,30 @@ long long avirb200_host_workspace_bytes(int mirror, int res_bits, int src_bits, 
     o.op = kWorkspace;
     if (run0(a, o) != 0) return -1;
     return (long long)o.bytes;
+}
+
+// avir::CImageResizer<fpclass>::resizeImageWindow (host buffers: the whole source in, the window out) and
+// resizeImageWindowDevice (d_src: the window's footprint), windowFootprint and windowWorkspaceBytes.
+// op: 0 host, 1 device, 2 footprint (info: 6 ints, avirb200_window_info), 3 workspace bytes (*bytes).
+int avirb200_host_window(int op, int mirror, int res_bits, int src_bits, int params_id, int tin, int tout,
+                         const void* src, int sw, int sh, int src_pitch, void* dst, int nw, int nh, int ch, double k,
+                         double ox, double oy, int gamma, int alpha, int build_mode, int wx, int wy, int ww, int wh,
+                         void* d_workspace, void* stream, int* info, long long* bytes) {
+    const CallArgs a{mirror, res_bits, src_bits, params_id, tin, tout, sw, sh, nw, nh, ch,
+                     k, ox, oy, gamma, alpha, build_mode};
+    static const Op ops[] = {kWinHost, kWinDevice, kWinFootprint, kWinWorkspace};
+    if (op < 0 || op > 3) {
+        g_err = "avirb200_host_window: op outside 0..3";
+        return -1;
+    }
+    OpArgs o{};
+    o.op = ops[op]; o.src = src; o.src_pitch = (size_t)src_pitch; o.dst = dst;
+    o.workspace = d_workspace; o.stream = stream;
+    o.wx = wx; o.wy = wy; o.ww = ww; o.wh = wh;
+    const int r = run0(a, o);
+    if (r == 0 && info != nullptr) std::memcpy(info, &o.info, sizeof o.info);
+    if (r == 0 && bytes != nullptr) *bytes = (long long)o.bytes;
+    return r;
 }
 
 } // extern "C"

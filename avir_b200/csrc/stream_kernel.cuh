@@ -505,7 +505,7 @@ AVS_FN void loader_init(const StreamParams& p, WarpRun<C, IS_V>& w) {
             constexpr int LSTEP = 32 / C::POSW; // lines one pass of the lanes covers
             const int pos = lane & (C::POSW - 1), lsub = lane / C::POSW;
             w.gp[k] = src + (size_t)(w.line0 + imin_(lsub + LSTEP * k, w.nlines - 1)) * rowb +
-                      (ptrdiff_t)(w.o0 - C::POSW + pos) * PIXB;
+                      (ptrdiff_t)(w.o0 - C::POSW + pos - p.src_row_base) * PIXB;
         }
     }
 }
@@ -571,7 +571,8 @@ AVS_FN void load_group(const StreamParams& p, WarpRun<C, IS_V>& w, int g, int gs
 #pragma unroll
                 for (int k = 0; k < NK; ++k) {
                     const int line = imin_(lsub + LSTEP * k, w.nlines - 1);
-                    cp_async_px<PIXB>(d + LSTEP * k * C::LINE_B, src + (size_t)(w.line0 + line) * rowb + (size_t)x * PIXB);
+                    cp_async_px<PIXB>(d + LSTEP * k * C::LINE_B,
+                                      src + (size_t)(w.line0 + line) * rowb + (size_t)(x - p.src_row_base) * PIXB);
                 }
             }
         }
@@ -690,7 +691,7 @@ AVS_FN void sink_h_store(const StreamParams& p, WarpRun<C, false>& w) {
     const int j = w.pend_j0 + pos;
     float* dst = static_cast<float*>(p.dst);
     const bool jok = (w.pend_j0 != kNoPend) && (j >= p.out0) && (j < p.out1);
-    float4* g = reinterpret_cast<float4*>(dst + (size_t)(w.line0 + lsub) * (size_t)p.dst_pitch) + j;
+    float4* g = reinterpret_cast<float4*>(dst + (size_t)(w.line0 + lsub) * (size_t)p.dst_pitch) + (j - p.dst_row_base);
     const size_t gstep = (size_t)(32 / M) * (size_t)(p.dst_pitch / 4);
 #pragma unroll
     for (int k = 0; k < M / 2; ++k) {
@@ -701,7 +702,8 @@ AVS_FN void sink_h_store(const StreamParams& p, WarpRun<C, false>& w) {
         // fused halo exchange: the lines [xs_l0, xs_l1) of this strip (empty outside the first / last strips of
         // a sharded band) also go straight into a neighbour's mailbox -- peer memory over NVLink, xs_delta
         // bytes from the line's own address.  Predicated stores, no branch: the loop stays straight-line.
-        unsigned char* ga = reinterpret_cast<unsigned char*>(reinterpret_cast<float4*>(dst + (size_t)(w.line0 + lsub) * (size_t)p.dst_pitch) + j) + w.xs_delta;
+        unsigned char* ga = reinterpret_cast<unsigned char*>(reinterpret_cast<float4*>(dst + (size_t)(w.line0 + lsub) * (size_t)p.dst_pitch) +
+                                                             (j - p.dst_row_base)) + w.xs_delta;
 #pragma unroll
         for (int k = 0; k < M / 2; ++k) {
             const int l = lsub + (32 / M) * k;

@@ -49,15 +49,18 @@ struct StreamParams {
     const float* srgb_lut; // kSrcU8Srgb: upstream's 256-entry linearisation table (device memory)
     float in_gamma_mult;   // kSrcU8Srgb: multiplier of the alpha channel
     long long src_pitch;  // elements between rows
-    int src_row_base;     // column pass: global row held by source row 0 (shards)
-    // Source positions the buffer actually holds, [src_lo, src_hi) (the whole line, or a shard's
-    // band of intermediate rows).  A run starts and ends on round boundaries, so its first / last
-    // round may compute outputs outside [out0, out1) (never stored) whose windows reach past the
-    // band: reads clamp to this range, not just to the line.
+    // Global source position held by the buffer's position 0: column pass, the intermediate row of a
+    // shard's or a window's first row; row pass, the source column of a window's footprint's first column.
+    int src_row_base;
+    // Source positions the buffer actually holds, [src_lo, src_hi) (the whole line, a shard's band of
+    // intermediate rows or a window's footprint columns).  A run starts and ends on round boundaries, so
+    // its first / last round may compute outputs outside [out0, out1) (never stored) whose windows reach
+    // past the band: reads clamp to this range, not just to the line.
     int src_lo, src_hi;
     void* dst;
     long long dst_pitch;
-    int dst_type, dst_row_base;
+    int dst_type;
+    int dst_row_base;     // final output stored at the destination's position 0 (row, or row-pass column)
     int gamma_out, alpha_index;
     float out_gamma_mult;
     int round_mode;
@@ -279,12 +282,20 @@ inline void stream_fill_params(StreamParams& p, const StreamAxisPlan& ap, const 
     p.pk_out = d.pk_out;
 }
 
+// Output columns of a row pass and the source columns its buffer holds: intermediate columns
+// [out0, out1) (stored from the intermediate's column 0 on) from a source buffer whose column 0 is
+// source column src_lo and that holds columns [src_lo, src_hi).  The whole line: {0, dst_w, 0, src_w}.
+struct StreamColumns {
+    int out0, out1, src_lo, src_hi;
+};
+
 // Row pass: every output column of `rows` source rows from `src` into the intermediate rows at `mid`
 // (pitches in elements).  seg_top / seg_bot: only the first seg_top and the last seg_bot of those rows,
-// in one launch (seg_bot > 0: two line segments).
+// in one launch (seg_bot > 0: two line segments).  cols: only those columns (a window), else all.
 inline void stream_fill_row_params(StreamParams& p, const StreamAxisPlan& ap, const avirb200_plan_desc& d,
                                    const void* src, long long src_pitch, float* mid, long long mid_pitch, int rows,
-                                   const float* lut, int seg_top = 0, int seg_bot = 0) {
+                                   const float* lut, int seg_top = 0, int seg_bot = 0,
+                                   const StreamColumns* cols = nullptr) {
     stream_fill_params(p, ap, d);
     p.n_lines = rows;
     if (seg_bot > 0) {
@@ -296,6 +307,13 @@ inline void stream_fill_row_params(StreamParams& p, const StreamAxisPlan& ap, co
     }
     p.out0 = 0;
     p.out1 = d.dst_w;
+    if (cols != nullptr) {
+        p.out0 = cols->out0;
+        p.out1 = cols->out1;
+        p.dst_row_base = cols->out0;
+        p.src_lo = p.src_row_base = cols->src_lo;
+        p.src_hi = cols->src_hi;
+    }
     p.src = src;
     p.src_type = stream_row_source_code(d);
     p.srgb_lut = lut;

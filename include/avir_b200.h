@@ -408,6 +408,77 @@ public:
                            "resizeImageDeviceBatch");
     }
 
+    // GPU extension: a destination WINDOW -- the pixels [WinX, WinX + WinWidth) x [WinY, WinY + WinHeight)
+    // of the NewWidth x NewHeight image resizeImage() makes of the same source, bit-identical to them --
+    // computed from the window's source footprint only.  The window is a call argument, not part of the
+    // plan: every window of one resize shares its cached plan.  SrcBuf is the WHOLE source image (only the
+    // footprint is read); NewBuf receives WinWidth x WinHeight pixels.  Error-diffusion classes throw.
+    template <typename Tin, typename Tout>
+    void resizeImageWindow(const Tin* const SrcBuf, const int SrcWidth, const int SrcHeight, int SrcScanlineSize,
+                           Tout* const NewBuf, const int NewWidth, const int NewHeight, const int ElCountIO,
+                           const double k, const int WinX, const int WinY, const int WinWidth, const int WinHeight,
+                           CImageResizerVars* const aVars = nullptr) const {
+        CImageResizerVars DefVars;
+        CImageResizerVars& Vars = (aVars == nullptr ? DefVars : *aVars);
+        if (SrcScanlineSize < 1) SrcScanlineSize = SrcWidth * ElCountIO;
+        std::shared_ptr<b200_detail::PlanHolder> ph = getWindowPlan<Tin, Tout>(SrcWidth, SrcHeight, NewWidth, NewHeight,
+                                                                                ElCountIO, k, Vars, "resizeImageWindow");
+        b200_detail::check(avirb200_resize_window_host(ph->dev, WinX, WinY, WinWidth, WinHeight, SrcBuf,
+                                                       (size_t)SrcScanlineSize, NewBuf, (size_t)WinWidth * ElCountIO),
+                           "resizeImageWindow");
+    }
+
+    // The same with DEVICE pointers, asynchronous on Vars.Stream: dSrcBuf points at the footprint's first
+    // pixel (windowFootprint()) and holds its src_w x src_h pixels, SrcScanlineSize elements apart (< 1:
+    // src_w * ElCountIO); `Workspace` holds windowWorkspaceBytes() bytes of device memory.
+    template <typename Tin, typename Tout>
+    void resizeImageWindowDevice(const Tin* const dSrcBuf, const int SrcWidth, const int SrcHeight,
+                                 int SrcScanlineSize, Tout* const dNewBuf, const int NewWidth, const int NewHeight,
+                                 const int ElCountIO, const double k, const int WinX, const int WinY,
+                                 const int WinWidth, const int WinHeight, void* const Workspace,
+                                 CImageResizerVars* const aVars = nullptr) const {
+        CImageResizerVars DefVars;
+        CImageResizerVars& Vars = (aVars == nullptr ? DefVars : *aVars);
+        std::shared_ptr<b200_detail::PlanHolder> ph = getWindowPlan<Tin, Tout>(
+            SrcWidth, SrcHeight, NewWidth, NewHeight, ElCountIO, k, Vars, "resizeImageWindowDevice");
+        avirb200_window_info wi;
+        b200_detail::check(avirb200_window_query(ph->dev, WinX, WinY, WinWidth, WinHeight, &wi), "resizeImageWindowDevice");
+        if (SrcScanlineSize < 1) SrcScanlineSize = wi.src_w * ElCountIO;
+        b200_detail::check(avirb200_resize_window_device(ph->dev, WinX, WinY, WinWidth, WinHeight, dSrcBuf,
+                                                         (size_t)SrcScanlineSize, dNewBuf, (size_t)WinWidth * ElCountIO,
+                                                         Workspace, Vars.Stream),
+                           "resizeImageWindowDevice");
+    }
+
+    // The source pixels a window reads (clamped to the image) and the intermediate rows it needs.
+    template <typename Tin, typename Tout>
+    avirb200_window_info windowFootprint(const int SrcWidth, const int SrcHeight, const int NewWidth,
+                                         const int NewHeight, const int ElCountIO, const double k, const int WinX,
+                                         const int WinY, const int WinWidth, const int WinHeight,
+                                         CImageResizerVars* const aVars = nullptr) const {
+        CImageResizerVars DefVars;
+        CImageResizerVars& Vars = (aVars == nullptr ? DefVars : *aVars);
+        std::shared_ptr<b200_detail::PlanHolder> ph =
+            getWindowPlan<Tin, Tout>(SrcWidth, SrcHeight, NewWidth, NewHeight, ElCountIO, k, Vars, "windowFootprint");
+        avirb200_window_info wi;
+        b200_detail::check(avirb200_window_query(ph->dev, WinX, WinY, WinWidth, WinHeight, &wi), "windowFootprint");
+        return wi;
+    }
+
+    template <typename Tin, typename Tout>
+    size_t windowWorkspaceBytes(const int SrcWidth, const int SrcHeight, const int NewWidth, const int NewHeight,
+                                const int ElCountIO, const double k, const int WinX, const int WinY,
+                                const int WinWidth, const int WinHeight, CImageResizerVars* const aVars = nullptr) const {
+        CImageResizerVars DefVars;
+        CImageResizerVars& Vars = (aVars == nullptr ? DefVars : *aVars);
+        std::shared_ptr<b200_detail::PlanHolder> ph = getWindowPlan<Tin, Tout>(
+            SrcWidth, SrcHeight, NewWidth, NewHeight, ElCountIO, k, Vars, "windowWorkspaceBytes");
+        size_t b = 0;
+        b200_detail::check(avirb200_window_workspace_bytes(ph->dev, WinX, WinY, WinWidth, WinHeight, &b),
+                           "windowWorkspaceBytes");
+        return b;
+    }
+
     // GPU extension: per-object tuning options (see CImageResizerTuning).
     mutable CImageResizerTuning Tuning;
 
@@ -457,6 +528,16 @@ private:
         const CImageResizerTuning& t = b200_detail::default_tuning();
         for (int i = 0; i < 6; ++i) avirb200_plan_set_option(ph->dev, i, Tuning.opt[i] >= 0 ? Tuning.opt[i] : t.opt[i]);
         return ph;
+    }
+
+    // The plan of a window call: the whole resize's (windows need non-empty images).
+    template <typename Tin, typename Tout>
+    std::shared_ptr<b200_detail::PlanHolder>
+    getWindowPlan(const int SrcWidth, const int SrcHeight, const int NewWidth, const int NewHeight,
+                  const int ElCountIO, const double k, CImageResizerVars& Vars, const char* what) const {
+        if (SrcWidth < 1 || SrcHeight < 1 || NewWidth < 1 || NewHeight < 1)
+            throw std::runtime_error(std::string("avir_b200: ") + what + " needs non-empty images");
+        return getPlan<Tin, Tout>(SrcWidth, SrcHeight, NewWidth, NewHeight, ElCountIO, k, Vars);
     }
 };
 

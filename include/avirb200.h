@@ -167,6 +167,43 @@ int avirb200_resize_device_batch(const avirb200_plan* plan, int n, const void* c
                                  size_t src_pitch, void* const* d_dsts, size_t dst_pitch,
                                  void* d_workspace, void* stream);
 
+/* ---- destination windows ------------------------------------------------------------- */
+
+/* A window is the destination sub-rectangle [x0, x0 + w) x [y0, y0 + h) of the plan's full
+ * src_w x src_h -> dst_w x dst_h resize.  Its pixels are bit-identical to the same pixels of
+ * avirb200_resize_device on the whole image, and a call reads only the window's source
+ * footprint and filters only the intermediate the window needs.  Windows must be non-empty and
+ * lie inside the destination (AVIRB200_ERR_BAD_ARG, before any CUDA call); plans with
+ * error diffusion, whose every pixel depends on all pixels before it, return
+ * AVIRB200_ERR_UNSUPPORTED. */
+typedef struct avirb200_window_info {
+    int32_t src_x0, src_w;      /* source columns the window reads (clamped to the image: reads */
+    int32_t src_y0, src_h;      /*   past an edge replicate the edge), and source rows */
+    int32_t mid_row0, mid_rows; /* intermediate rows the column pass reads (= the source rows) */
+} avirb200_window_info;
+
+/* The footprint of a window.  Also builds the per-range device tables the window's passes use,
+ * so that avirb200_resize_window_device stays asynchronous and allocation-free. */
+int avirb200_window_query(const avirb200_plan* plan, int x0, int y0, int w, int h, avirb200_window_info* info);
+/* Same, from a descriptor alone (pure host arithmetic, no device needed). */
+int avirb200_window_query_desc(const avirb200_plan_desc* desc, int x0, int y0, int w, int h,
+                               avirb200_window_info* info);
+/* Workspace of one window call: the intermediate (mid_rows x w pixels of floats) and, where the
+ * plan uses them, the float copies of double buffers and the 4-channel copies of 1..3-channel
+ * images, sized for the footprint and the window. */
+int avirb200_window_workspace_bytes(const avirb200_plan* plan, int x0, int y0, int w, int h, size_t* bytes);
+/* d_src points at the footprint's first pixel (source pixel (src_x0, src_y0)) and holds the
+ * footprint's src_w x src_h pixels; d_dst points at the window's first pixel and receives w x h
+ * pixels.  Pitches in elements, as in avirb200_resize_device; the same stream rules (no
+ * allocation, no synchronisation). */
+int avirb200_resize_window_device(const avirb200_plan* plan, int x0, int y0, int w, int h, const void* d_src,
+                                  size_t src_pitch, void* d_dst, size_t dst_pitch, void* d_workspace,
+                                  void* stream);
+/* The same with HOST buffers: h_src is the WHOLE source image (only the footprint is copied to the
+ * device), h_dst receives the w x h window.  Pageable or page-locked memory; synchronises. */
+int avirb200_resize_window_host(avirb200_plan* plan, int x0, int y0, int w, int h, const void* h_src,
+                                size_t src_pitch, void* h_dst, size_t dst_pitch);
+
 /* Per-plan options (tuning and test switches; none changes a result bit).  Options are plan
  * state: set them while no call on the plan is in flight.  value < 0 restores the default. */
 typedef enum avirb200_option {

@@ -154,7 +154,8 @@ def build_emul(force=False):
 
 def _build_emul(force=False, name="stream_emul"):
     """TEST INFRASTRUCTURE: host lockstep emulation of the streaming kernel (tests/emul): lib<name>.so
-    from <name>.cpp (window_emul.cpp: the windowed passes, on stream_emul.cpp's emulation)."""
+    from <name>.cpp (window_emul.cpp: the windowed passes, on stream_emul.cpp's emulation; config_emul.cpp:
+    the generic kernel's shared-memory layout, pass_config.h)."""
     d = os.path.join(ROOT, "tests", "emul")
     target = os.path.join(d, "lib%s.so" % name)
     src = os.path.join(d, name + ".cpp")
@@ -174,12 +175,18 @@ def build_window_emul(force=False):
         return _build_emul(force, "window_emul")
 
 
+def build_config_emul(force=False):
+    with _BuildLock():
+        return _build_emul(force, "config_emul")
+
+
 def build_all(force=False, verbose=False):
     build_cuda(force, verbose)
     build_host(force)
     build_oracles()
     build_emul(force)
     build_window_emul(force)
+    build_config_emul(force)
 
 
 if __name__ == "__main__":

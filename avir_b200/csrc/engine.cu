@@ -30,6 +30,7 @@
 #include "fast_pass.cuh"
 #include "generic_pass.cuh"
 #include "host_util.h"
+#include "pass_config.h"
 #include "stream_types.h"
 #include "stream_launch.h"
 
@@ -69,14 +70,6 @@ void make_srgb_lut(float* lut) {
         lut[i] = f;
     }
 }
-
-struct PassConfig {
-    int lines_per_block = 0;
-    int tile_out = 0;
-    int span = 0;
-    int pitch = 0;
-    size_t smem = 0;
-};
 
 struct HostAxis {
     avirb200_axis_desc desc;              // pointers are HOST copies (below)
@@ -126,6 +119,7 @@ struct avirb200_plan {
     int opt_all_chains = 0;
     int opt_overlap = 3;      // sharded: how the halo rows travel (AVIRB200_OPT_OVERLAP_HALO; 3 = fused into the kernels)
     int sm_count = 132;       // of `device`
+    size_t smem_optin = 232448; // of `device`: the most dynamic shared memory one block may opt in to
     Halo* halo = nullptr; // sharded: peer mailboxes (created by the first sharded call)
     cudaStream_t stream_x = nullptr; // sharded: exchange stream
     cudaEvent_t ev_x0 = nullptr, ev_x1 = nullptr;
@@ -207,32 +201,6 @@ const T* stage(std::vector<char>& img, size_t& off, char* dbase, const std::vect
     return d;
 }
 
-// The kernels' view of an axis descriptor, with the descriptor's (host) table pointers: what the
-// range arithmetic reads.
-DevAxis host_axis_view(const avirb200_axis_desc& ad) {
-    DevAxis d;
-    std::memset(&d, 0, sizeof d);
-    d.src_len = ad.src_len; d.dst_len = ad.dst_len; d.nsteps = ad.nsteps;
-    int lo = 0, hi = ad.src_len;
-    for (int i = 0; i < ad.nsteps && i < AVIRB200_MAX_STEPS; ++i) {
-        const avirb200_step_desc& s = ad.steps[i];
-        DevStep& ds = d.steps[i];
-        ds.kind = s.kind; ds.resample = s.resample; ds.latency = s.latency; ds.edge = s.edge;
-        ds.in_len = s.in_len; ds.out_len = s.out_len; ds.ntaps = s.ntaps; ds.order = s.order;
-        ds.upsampled = s.upsampled; ds.skip_odd = s.skip_odd; ds.zero_start = s.zero_start;
-        ds.nphases = s.nphases;
-        ds.out_prefix = s.out_prefix; ds.out_suffix = s.out_suffix;
-        ds.in_prefix = s.in_prefix; ds.in_suffix = s.in_suffix;
-        ds.n_prefix_dc = s.n_prefix_dc; ds.n_suffix_dc = s.n_suffix_dc;
-        ds.in_lo = lo; ds.in_hi = hi;
-        ds.taps = s.taps; ds.src_pos = s.src_pos; ds.phase = s.phase; ds.frac = s.frac;
-        ds.prefix_dc = s.prefix_dc; ds.suffix_dc = s.suffix_dc;
-        const Range od = step_output_domain(ds);
-        lo = od.a; hi = od.b + 1;
-    }
-    return d;
-}
-
 // hostdev: the axis with the plan's host copies of the tables; dev: the same with the copies staged
 // into the plan's device arena.
 void build_dev_axis(HostAxis& ha, std::vector<char>& img, size_t& off, char* dbase) {
@@ -246,44 +214,6 @@ void build_dev_axis(HostAxis& ha, std::vector<char>& img, size_t& off, char* dba
         ds.prefix_dc = stage(img, off, dbase, ha.pdc[i]);
         ds.suffix_dc = stage(img, off, dbase, ha.sdc[i]);
     }
-}
-
-// Source range a final-output range needs, through the whole chain (host side).
-Range chain_source_range(const DevAxis& hd, Range out, int* max_span) {
-    Range r = out;
-    int span = r.b - r.a + 1;
-    for (int i = hd.nsteps - 1; i >= 0; --i) {
-        r = step_input_range(hd.steps[i], r, hd.steps[i].src_pos);
-        span = imax(span, r.b - r.a + 1);
-    }
-    if (max_span) *max_span = span;
-    return r;
-}
-
-const size_t kGenericSmemBudget = 100 * 1024;
-
-PassConfig choose_generic_config(const DevAxis& hd, int channels, int out0, int out1) {
-    PassConfig c;
-    c.lines_per_block = imax(1, 64 / channels);
-    c.pitch = (c.lines_per_block * channels) | 1;
-    static const int cand[] = {1024, 768, 512, 384, 256, 192, 128, 96, 64, 48, 32, 24, 16, 12, 8, 4, 2, 1};
-    for (int t : cand) {
-        int worst = 0;
-        for (int j0 = out0; j0 < out1; j0 += t) {
-            int sp = 0;
-            Range o{j0, imin(j0 + t, out1) - 1};
-            chain_source_range(hd, o, &sp);
-            worst = imax(worst, sp);
-        }
-        const size_t smem = 2ull * worst * c.pitch * sizeof(float);
-        if (smem <= kGenericSmemBudget || t == 1) {
-            c.tile_out = t;
-            c.span = worst;
-            c.smem = smem;
-            break;
-        }
-    }
-    return c;
 }
 
 void fill_common(PassParams& p, const avirb200_plan* pl) {
@@ -394,8 +324,9 @@ int run_row_pass(const avirb200_plan* pl, const void* d_src, size_t src_pitch, f
     PassParams p;
     std::memset(&p, 0, sizeof p);
     fill_common(p, pl);
-    const PassConfig c = (p4 || cols != nullptr) ? choose_generic_config(pl->h.hostdev, p4 ? 4 : d.channels, cr.out0, cr.out1)
-                                                 : pl->cfg_h;
+    const PassConfig c = (p4 || cols != nullptr)
+                             ? choose_generic_config(pl->h.hostdev, p4 ? 4 : d.channels, cr.out0, cr.out1, pl->smem_optin)
+                             : pl->cfg_h;
     if (p4) p.channels = 4;
     p.ax = pl->h.dev;
     p.is_v = 0;
@@ -404,7 +335,7 @@ int run_row_pass(const avirb200_plan* pl, const void* d_src, size_t src_pitch, f
     p.tile_out = c.tile_out;
     p.out0 = cr.out0;
     p.out1 = cr.out1;
-    p.span = c.span;
+    p.span_a = c.span_a;
     p.pitch = c.pitch;
     p.src = d_src;
     p.src_pitch = (long long)src_pitch;
@@ -476,12 +407,12 @@ int run_col_pass(const avirb200_plan* pl, const float* d_mid, int mid_row_base, 
     p.is_v = 1;
     p.n_lines = d.dst_w;
     PassConfig c = pl->cfg_v;
-    if (p4 || out0 != 0 || out1 != d.dst_h) c = choose_generic_config(pl->v.hostdev, p.channels, out0, out1);
+    if (p4 || out0 != 0 || out1 != d.dst_h) c = choose_generic_config(pl->v.hostdev, p.channels, out0, out1, pl->smem_optin);
     p.lines_per_block = c.lines_per_block;
     p.tile_out = c.tile_out;
     p.out0 = out0;
     p.out1 = out1;
-    p.span = c.span;
+    p.span_a = c.span_a;
     p.pitch = c.pitch;
     p.src = d_mid;
     p.src_pitch = (long long)mid_pitch(pl, d.dst_w);
@@ -1334,6 +1265,27 @@ int avirb200_plan_create(const avirb200_plan_desc* desc, avirb200_plan** out) {
     r = copy_axis_host(pl->v, desc->v);
     if (r != 0) return r;
     CUDA_TRY(cudaGetDevice(&pl->device));
+    {
+        int n = 0;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, pl->device) == cudaSuccess && n > 0)
+            pl->sm_count = n;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMaxSharedMemoryPerBlockOptin, pl->device) == cudaSuccess && n > 0)
+            pl->smem_optin = (size_t)n;
+    }
+    // The generic kernel runs every pass no other kernel takes (and every pass under KERNEL_FAMILY 1), so a
+    // plan whose pass does not fit it even as one output of one line per block is refused here, before any
+    // launch.  What remains are long lines to very few pixels: a 4-channel line of more than about 11 600
+    // source pixels to one pixel on an H100 (the source span of that one output, 5 floats per position).
+    pl->cfg_h = choose_generic_config(host_axis_view(pl->h.desc), desc->channels, 0, desc->dst_w, pl->smem_optin);
+    pl->cfg_v = choose_generic_config(host_axis_view(pl->v.desc), desc->channels, 0, desc->dst_h, pl->smem_optin);
+    for (int a = 0; a < 2; ++a) {
+        const PassConfig& c = a ? pl->cfg_v : pl->cfg_h;
+        if (c.smem > pl->smem_optin)
+            return fail(AVIRB200_ERR_UNSUPPORTED,
+                        std::string(a ? "column pass" : "row pass") + ": one output of one line needs " +
+                            std::to_string(c.smem) + " bytes of shared memory, more than the " +
+                            std::to_string(pl->smem_optin) + " a block of this device can have");
+    }
 
     const size_t bytes = axis_arena_bytes(pl->h) + axis_arena_bytes(pl->v) + 1024 + 256;
     CUDA_TRY(cudaMalloc(&pl->arena, bytes));
@@ -1350,8 +1302,6 @@ int avirb200_plan_create(const avirb200_plan_desc* desc, avirb200_plan** out) {
     build_dev_axis(pl->v, img, off, static_cast<char*>(pl->arena));
     CUDA_TRY(cudaMemcpy(pl->arena, img.data(), bytes, cudaMemcpyHostToDevice));
 
-    pl->cfg_h = choose_generic_config(pl->h.hostdev, desc->channels, 0, desc->dst_w);
-    pl->cfg_v = choose_generic_config(pl->v.hostdev, desc->channels, 0, desc->dst_h);
     // (pl->desc, not *desc: the kernels' element types, see io_in_type / io_out_type)
     // 1..3 channels: can both passes run on the 4-channel kernels (widened copies)?  Not for plans
     // with double buffers or error diffusion (they keep the image's own channel count throughout).
@@ -1373,11 +1323,6 @@ int avirb200_plan_create(const avirb200_plan_desc* desc, avirb200_plan** out) {
             pl->stream_h.chain = pl->stream_v.chain = 0;
             pl->fast.h_ok = pl->fast.v_ok = false;
         }
-    }
-    {
-        int n = 0;
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, pl->device) == cudaSuccess && n > 0)
-            pl->sm_count = n;
     }
     *out = pl.release();
     return 0;

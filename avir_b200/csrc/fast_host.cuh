@@ -250,6 +250,9 @@ inline void fast_plan_init(FastPlan& f, const DevAxis& h_host, const DevAxis& v_
         if (fast_upload(fp) != 0) continue;
         fp.raw = (a == 0 && d.in_type != AVIRB200_F32);
         fast_choose_tile(fp, 0, hs[a]->dst_len);
+        // a footprint beyond the budget even at the shortest tile (large downscale ratios: the source
+        // span of one output grows with the ratio) leaves the pass to the generic kernel
+        if (fp.fpnt.smem > kFastSmemBudget) continue;
         // the whole-image tile table is built and uploaded here, not at the first launch (launches
         // stay asynchronous and allocation-free; shard ranges: fast_prepare_range())
         fp.ok = (fast_tile_table(fp, 0, hs[a]->dst_len) != nullptr);

@@ -35,7 +35,7 @@ struct PassParams {
     int lines_per_block;
     int tile_out;   // final outputs per tile
     int out0, out1; // final outputs [out0, out1) to produce (column pass on a shard, either pass of a window)
-    int span;       // shared rows per buffer
+    int span_a;     // shared rows of buffer 0 (buffer 1 follows it; pass_config.h)
     int pitch;      // shared row pitch in floats (odd)
     // source image / intermediate
     const void* src;
@@ -209,7 +209,7 @@ template <int SUM>
 __global__ void __launch_bounds__(256)
 generic_pass_kernel(const __grid_constant__ PassParams p) {
     extern __shared__ float smem[];
-    float* bufs[2] = {smem, smem + (size_t)p.span * p.pitch};
+    float* bufs[2] = {smem, smem + (size_t)p.span_a * p.pitch};
 
     const int C = p.channels;
     const int line0 = blockIdx.y * p.lines_per_block;

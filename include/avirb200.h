@@ -123,7 +123,13 @@ typedef struct avirb200_plan avirb200_plan; /* opaque, device-resident tables */
 
 /* ---- single-GPU path --------------------------------------------------------------- */
 
-/* Copies the descriptor's tables to the current CUDA device. */
+/* Copies the descriptor's tables to the current CUDA device.
+ * Every pass must fit the generic kernel with one output of one line per block: the source span of
+ * that output (about 19 x the downscale ratio on the axis, at most the line) times (channels | 1)
+ * floats, in the device's opt-in shared memory per block.  A plan that does not fit is refused here
+ * with AVIRB200_ERR_UNSUPPORTED and a message naming the pass; no call of a created plan fails for
+ * this reason.  On an H100 (227 KiB per block) this refuses only 4-channel lines of more than about
+ * 11 600 source pixels resized to very few pixels (e.g. 16384 x 4 -> 1 x 4 RGBA). */
 int avirb200_plan_create(const avirb200_plan_desc* desc, avirb200_plan** out);
 void avirb200_plan_destroy(avirb200_plan* plan);
 

@@ -38,6 +38,31 @@ struct Range {
     int a, b; // inclusive
 };
 
+// What every kernel family does to a pixel on the way in (sRGB linearisation: row pass) and on the way out
+// (gamma, rounding, bit-depth truncation, clamping: column pass).
+struct PixelStage {
+    int gamma_in, gamma_out, alpha_index;
+    float in_gamma_mult, out_gamma_mult;
+    const float* srgb_lut; // 256 floats (u8 input), device memory
+    int round_mode;
+    float tr_mul, tr_mul_inv, pk_out;
+};
+
+inline PixelStage pixel_stage(const avirb200_plan_desc& d, const float* srgb_lut) {
+    PixelStage s;
+    s.gamma_in = (d.use_gamma & 1) ? 1 : 0;
+    s.gamma_out = (d.use_gamma & 2) ? 1 : 0;
+    s.alpha_index = d.alpha_index;
+    s.in_gamma_mult = d.in_gamma_mult;
+    s.out_gamma_mult = d.out_gamma_mult;
+    s.srgb_lut = srgb_lut;
+    s.round_mode = d.round_mode;
+    s.tr_mul = d.tr_mul;
+    s.tr_mul_inv = d.tr_mul_inv;
+    s.pk_out = d.pk_out;
+    return s;
+}
+
 AVB_HD int floordiv(int a, int b) { return (a >= 0) ? a / b : -((-a + b - 1) / b); }
 AVB_HD int imin(int a, int b) { return a < b ? a : b; }
 AVB_HD int imax(int a, int b) { return a > b ? a : b; }

@@ -31,6 +31,7 @@
 #include "generic_pass.cuh"
 #include "host_util.h"
 #include "pass_config.h"
+#include "pass_request.h"
 #include "stream_types.h"
 #include "stream_launch.h"
 
@@ -216,22 +217,6 @@ void build_dev_axis(HostAxis& ha, std::vector<char>& img, size_t& off, char* dba
     }
 }
 
-void fill_common(PassParams& p, const avirb200_plan* pl) {
-    const avirb200_plan_desc& d = pl->desc;
-    p.sum_mode = d.sum_mode;
-    p.channels = d.channels;
-    p.gamma_in = (d.use_gamma & 1) ? 1 : 0;
-    p.gamma_out = (d.use_gamma & 2) ? 1 : 0;
-    p.alpha_index = d.alpha_index;
-    p.in_gamma_mult = d.in_gamma_mult;
-    p.out_gamma_mult = d.out_gamma_mult;
-    p.srgb_lut = pl->d_lut;
-    p.round_mode = d.round_mode;
-    p.tr_mul = d.tr_mul;
-    p.tr_mul_inv = d.tr_mul_inv;
-    p.pk_out = d.pk_out;
-}
-
 int launch_generic(const PassParams& p, const PassConfig& c, cudaStream_t st) {
     dim3 grid((p.out1 - p.out0 + c.tile_out - 1) / c.tile_out,
               (p.n_lines + c.lines_per_block - 1) / c.lines_per_block);
@@ -262,169 +247,126 @@ size_t mid_pitch(const avirb200_plan* pl, int cols = -1) {
     return (size_t)(cols >= 0 ? cols : pl->desc.dst_w) * pl->mid_ch;
 }
 
-// Whether a pass runs on the streaming kernel with these buffers (the kernel's source / destination as
-// it sees them: a widened plan's scratch copies).  The copies move whole pixels: the row pass's source
-// pixels and the column pass's channel pairs must be aligned to their size, the intermediate to 16 bytes.
-bool row_pass_on_stream(const avirb200_plan* pl, const void* src, size_t src_pitch, const float* mid) {
-    return pl->opt_family == 0 && pl->stream_h.chain != 0 && ((uintptr_t)src % (4 * elem_size(pl->desc.in_type))) == 0 &&
-           (src_pitch % 4) == 0 && ((uintptr_t)mid % 16) == 0;
-}
-bool col_pass_on_stream(const avirb200_plan* pl, const void* dst, size_t dst_pitch, const float* mid) {
-    return pl->opt_family == 0 && pl->stream_v.chain != 0 && ((uintptr_t)dst % (2 * elem_size(pl->desc.out_type))) == 0 &&
-           (dst_pitch % 2) == 0 && ((uintptr_t)mid % 16) == 0;
+enum PassFamily { kFamilyStream, kFamilyTile, kFamilyGeneric };
+
+struct PassRoute {
+    PassFamily family;
+    PassRequest k;      // the request as the kernels see it: a widened plan's scratch copies
+    FastFootprint fpnt; // kFamilyTile: the footprint of the request's range
+};
+
+// The kernel family that runs the pass `req`: the first that applies of the streaming kernel, the tile
+// kernel and the generic kernel.  The 4-channel kernels (streaming, tile) move whole pixels: the row pass's
+// source pixels and the column pass's channel pairs must be aligned to their size, the intermediate to 16
+// bytes.  The tile kernel also needs the footprint of the request's tiles to fit its shared memory.
+PassRoute pass_family(const avirb200_plan* pl, const PassRequest& req) {
+    PassRoute r;
+    r.k = req;
+    PassRequest& k = r.k;
+    if (use_pad4(pl)) {
+        if (k.is_v) {
+            k.dst = k.scratch4;
+            k.dst_pitch = (size_t)k.lines * 4;
+        } else {
+            k.src = k.scratch4;
+            k.src_pitch = (size_t)(k.src_hi - k.src_lo) * 4;
+        }
+    }
+    const bool aligned = k.is_v ? ((uintptr_t)k.dst % (2 * elem_size(k.dst_type))) == 0 && (k.dst_pitch % 2) == 0 &&
+                                      ((uintptr_t)k.src % 16) == 0
+                                : ((uintptr_t)k.src % (4 * elem_size(k.src_type))) == 0 && (k.src_pitch % 4) == 0 &&
+                                      ((uintptr_t)k.dst % 16) == 0;
+    const avs::StreamAxisPlan& sa = k.is_v ? pl->stream_v : pl->stream_h;
+    const bool tile_ok = k.is_v ? pl->fast.v_ok : pl->fast.h_ok;
+    if (pl->opt_family == 0 && sa.chain != 0 && aligned) {
+        r.family = kFamilyStream;
+    } else if (pl->opt_family != 1 && tile_ok && aligned &&
+               (r.fpnt = fast_range_footprint(k.is_v ? pl->fast.v : pl->fast.h, k.out0, k.out1)).smem <= kFastSmemBudget) {
+        r.family = kFamilyTile;
+    } else {
+        r.family = kFamilyGeneric;
+    }
+    return r;
 }
 
-// Row pass over `rows` source rows (band starting at d_src) into the intermediate band
-// starting at d_mid; column pass producing dst rows [out0, out1) from an intermediate
-// buffer whose row 0 is global row mid_row_base.
-// scratch4: where the band's widened (4-channel) copy goes when use_pad4(pl).
-// seg_top / seg_bot (4-channel plans only, the caller checks row_pass_on_stream()): filter only the
-// band's first seg_top and last seg_bot rows, in ONE launch.
-// xs (sharded calls, fused halo exchange): the band's link, sent through the streaming kernel; *xs_done
-// tells whether the streaming kernel took the pass (and so delivered the neighbours' rows).
-// cols (windows): only the intermediate columns [out0, out1), stored from d_mid's column 0 on, from a
-// source buffer whose column 0 is source column src_lo and that holds columns [src_lo, src_hi); null:
-// every column of the whole source line.
-int run_row_pass(const avirb200_plan* pl, const void* d_src, size_t src_pitch, float* d_mid,
-                 int rows, cudaStream_t st, int* launches, void* scratch4 = nullptr, int seg_top = 0, int seg_bot = 0,
-                 const avs::StreamLink* xs = nullptr, bool* xs_done = nullptr, const avs::StreamColumns* cols = nullptr) {
-    if (rows <= 0) return 0;
+// The generic kernel's parameters of the pass k (its buffers as the kernel sees them), `channels` wide: the
+// plan's cached layout for a whole pass at the image's channel count, else the range's own.
+int generic_pass(const avirb200_plan* pl, const PassRequest& k, int channels, cudaStream_t st) {
+    const avirb200_plan_desc& d = pl->desc;
+    const HostAxis& ax = k.is_v ? pl->v : pl->h;
+    const PassConfig c = (channels == d.channels && k.out0 == 0 && k.out1 == ax.desc.dst_len)
+                             ? (k.is_v ? pl->cfg_v : pl->cfg_h)
+                             : choose_generic_config(ax.hostdev, channels, k.out0, k.out1, pl->smem_optin);
+    PassParams p;
+    std::memset(&p, 0, sizeof p);
+    p.ax = ax.dev;
+    p.sum_mode = d.sum_mode;
+    p.is_v = k.is_v ? 1 : 0;
+    p.channels = channels;
+    p.n_lines = k.lines;
+    p.lines_per_block = c.lines_per_block;
+    p.tile_out = c.tile_out;
+    p.out0 = k.out0;
+    p.out1 = k.out1;
+    p.span_a = c.span_a;
+    p.pitch = c.pitch;
+    p.src = k.src;
+    p.src_pitch = (long long)k.src_pitch;
+    p.src_type = k.src_type;
+    p.src_row_base = k.src_base;
+    p.dst = k.dst;
+    p.dst_pitch = (long long)k.dst_pitch;
+    p.dst_type = k.dst_type;
+    p.dst_row_base = k.dst_base;
+    p.px = pixel_stage(d, pl->d_lut);
+    return launch_generic(p, c, st);
+}
+
+// Runs one pass on the family pass_family() picks.  A widened plan's row pass first widens the source
+// into req.scratch4, its column pass writes 4-channel pixels there and narrows them into req.dst; a widened
+// pass the 4-channel kernels do not take runs the generic kernel with 4 channels (the pad channel's results
+// are dropped).  Line segments and links are the streaming kernel's: the caller asks pass_family() first.
+int run_pass(const avirb200_plan* pl, const PassRequest& req, cudaStream_t st, int* launches) {
+    if (req.lines <= 0 || req.out1 <= req.out0) return 0;
     // (a non-sticky error another library left in this thread -- NCCL's peer-access probing leaves
     // cudaErrorPeerAccessAlreadyEnabled once the IPC mailboxes have enabled it -- is not this launch's)
     (void)cudaGetLastError();
     const avirb200_plan_desc& d = pl->desc;
-    const avs::StreamColumns cr = cols ? *cols : avs::StreamColumns{0, d.dst_w, 0, d.src_w};
-    const size_t mp = mid_pitch(pl, cr.out1 - cr.out0);
+    const char* pass = req.is_v ? "column pass" : "row pass";
     const bool p4 = use_pad4(pl);
-    if (p4) {
-        if (scratch4 == nullptr) return fail(AVIRB200_ERR_BAD_ARG, "row pass: no scratch for the widened source");
-        if (launch_widen(d.in_type, d_src, src_pitch, scratch4, cr.src_hi - cr.src_lo, rows, d.channels, st) != 0)
+    if (p4 && req.scratch4 == nullptr) return fail(AVIRB200_ERR_BAD_ARG, std::string(pass) + ": no scratch for the widened pixels");
+    const PassRoute r = pass_family(pl, req);
+    const PassRequest& k = r.k;
+    if ((k.link != nullptr || k.seg_top > 0 || k.seg_bot > 0) && r.family != kFamilyStream)
+        return fail(AVIRB200_ERR_BAD_ARG, std::string(pass) + ": line segments and links need the streaming kernel");
+    if (p4 && !k.is_v) {
+        if (launch_widen(d.in_type, req.src, req.src_pitch, req.scratch4, k.src_hi - k.src_lo, k.lines, d.channels, st) != 0)
             return fail(AVIRB200_ERR_CUDA, "widening the source failed");
         ++*launches;
-        d_src = scratch4;
-        src_pitch = (size_t)(cr.src_hi - cr.src_lo) * 4;
     }
-    if (row_pass_on_stream(pl, d_src, src_pitch, d_mid)) {
+    int e = 0;
+    if (r.family == kFamilyStream) {
+        const avs::StreamAxisPlan& sa = k.is_v ? pl->stream_v : pl->stream_h;
         avs::StreamParams sp;
-        avs::stream_fill_row_params(sp, pl->stream_h, d, d_src, (long long)src_pitch, d_mid, (long long)mp, rows,
-                                    pl->d_lut, seg_top, seg_bot, cols);
-        if (xs != nullptr) avs::stream_set_sender(sp, *xs);
-        const int r = avs::stream_launch(pl->stream_h.chain, false, 0, pl->opt_var_h, sp, pl->sm_count, st);
-        if (r == -1) return fail(AVIRB200_ERR_CUDA, "streaming row pass launch failed");
-        if (r == 0) { ++*launches; if (xs_done) *xs_done = (xs != nullptr); return 0; }
+        avs::stream_params(sp, sa, d, k, pl->d_lut);
+        if (avs::stream_launch(sa.chain, k.is_v, avs::stream_epilogue_code(d), k.is_v ? pl->opt_var_v : pl->opt_var_h, sp,
+                               pl->sm_count, st) != 0)
+            e = fail(AVIRB200_ERR_CUDA, std::string("streaming ") + pass + " launch failed");
+    } else if (r.family == kFamilyTile) {
+        if (fast_pass(k.is_v ? pl->fast.v : pl->fast.h, k, r.fpnt, pixel_stage(d, pl->d_lut), d.sum_mode, pl->sm_count,
+                      st) != 0)
+            e = fail(AVIRB200_ERR_CUDA, std::string("fast ") + pass + " launch failed");
+    } else {
+        e = generic_pass(pl, k, p4 ? 4 : d.channels, st);
     }
-    if (pl->opt_family != 1 && pl->fast.h_ok) {
-        const int r = fast_row_pass(pl->fast, d, d_src, src_pitch, d_mid, mp, rows, pl->d_lut, pl->sm_count, st,
-                                    cr.out0, cr.out1, cr.src_lo);
-        if (r == -1) return fail(AVIRB200_ERR_CUDA, "fast row pass launch failed");
-        if (r == 0) { ++*launches; return 0; }
-    }
-    // The generic kernel.  A widened band the 4-channel kernels did not take runs it on the widened
-    // copy with 4 channels (the pad channel's results are dropped).
-    PassParams p;
-    std::memset(&p, 0, sizeof p);
-    fill_common(p, pl);
-    const PassConfig c = (p4 || cols != nullptr)
-                             ? choose_generic_config(pl->h.hostdev, p4 ? 4 : d.channels, cr.out0, cr.out1, pl->smem_optin)
-                             : pl->cfg_h;
-    if (p4) p.channels = 4;
-    p.ax = pl->h.dev;
-    p.is_v = 0;
-    p.n_lines = rows;
-    p.lines_per_block = c.lines_per_block;
-    p.tile_out = c.tile_out;
-    p.out0 = cr.out0;
-    p.out1 = cr.out1;
-    p.span_a = c.span_a;
-    p.pitch = c.pitch;
-    p.src = d_src;
-    p.src_pitch = (long long)src_pitch;
-    p.src_type = d.in_type;
-    p.src_row_base = cr.src_lo;
-    p.dst = d_mid;
-    p.dst_pitch = (long long)mp;
-    p.dst_type = AVIRB200_F32;
-    p.dst_row_base = cr.out0;
+    if (e != 0) return e;
     ++*launches;
-    return launch_generic(p, c, st);
-}
-
-// scratch4: where the band's 4-channel destination rows go when use_pad4(pl) (then narrowed into d_dst).
-// mid_rows: intermediate rows the buffer holds from mid_row_base on (< 0: up to the image's last row).
-// xr (sharded calls, fused halo exchange): the band's link -- the neighbours' rows are read in place from
-// its mailbox.  Returns 1, nothing launched, when the streaming kernel cannot take the pass (the caller
-// moves the rows into the workspace and calls again without xr).
-// cols (windows): pixel columns of the intermediate and the destination (< 0: the destination width).
-int run_col_pass(const avirb200_plan* pl, const float* d_mid, int mid_row_base, void* d_dst,
-                 size_t dst_pitch, int out0, int out1, cudaStream_t st, int* launches, void* scratch4 = nullptr,
-                 int mid_rows = -1, const avs::StreamLink* xr = nullptr, int cols = -1) {
-    if (out1 <= out0) return 0;
-    (void)cudaGetLastError(); // (see run_row_pass)
-    // (a window's column pass is the whole image's on a narrower intermediate: dst_w = its columns)
-    avirb200_plan_desc d = pl->desc;
-    if (cols >= 0) d.dst_w = cols;
-    const bool p4 = use_pad4(pl);
-    void* const user_dst = d_dst;
-    const size_t user_pitch = dst_pitch;
-    if (p4) {
-        if (scratch4 == nullptr) return fail(AVIRB200_ERR_BAD_ARG, "column pass: no scratch for the 4-channel destination");
-        d_dst = scratch4;
-        dst_pitch = (size_t)d.dst_w * 4;
-    }
-    auto finish = [&]() -> int {
-        if (!p4) return 0;
-        if (launch_narrow(d.out_type, scratch4, user_dst, user_pitch, d.dst_w, out1 - out0, d.channels, st) != 0)
+    if (p4 && k.is_v) {
+        if (launch_narrow(d.out_type, k.dst, req.dst, req.dst_pitch, k.lines, k.out1 - k.out0, d.channels, st) != 0)
             return fail(AVIRB200_ERR_CUDA, "narrowing the destination failed");
         ++*launches;
-        return 0;
-    };
-    if (col_pass_on_stream(pl, d_dst, dst_pitch, d_mid)) {
-        avs::StreamParams sp;
-        avs::stream_fill_col_params(sp, pl->stream_v, d, d_mid, (long long)mid_pitch(pl, d.dst_w), mid_row_base,
-                                    (mid_rows >= 0) ? mid_row_base + mid_rows : d.src_h, d_dst, (long long)dst_pitch,
-                                    out0, out1);
-        if (xr != nullptr) avs::stream_set_receiver(sp, *xr);
-        const int r = avs::stream_launch(pl->stream_v.chain, true, avs::stream_epilogue_code(d), pl->opt_var_v, sp,
-                                         pl->sm_count, st);
-        if (r == -1) return fail(AVIRB200_ERR_CUDA, "streaming column pass launch failed");
-        if (r == 0) { ++*launches; return finish(); }
     }
-    if (xr != nullptr) return 1;
-    if (pl->opt_family != 1 && pl->fast.v_ok) {
-        const int r = fast_col_pass(pl->fast, d, d_mid, mid_pitch(pl, d.dst_w), mid_row_base, d_dst, dst_pitch, out0, out1,
-                                    pl->d_lut, pl->sm_count, st);
-        if (r == -1) return fail(AVIRB200_ERR_CUDA, "fast column pass launch failed");
-        if (r == 0) { ++*launches; return finish(); }
-    }
-    // The generic kernel.  A widened band the tile kernel refused (a shard whose footprint exceeds its
-    // shared memory) runs it with 4 channels into the 4-channel scratch, narrowed as after the
-    // 4-channel kernels.
-    PassParams p;
-    std::memset(&p, 0, sizeof p);
-    fill_common(p, pl);
-    if (p4) p.channels = 4;
-    p.ax = pl->v.dev;
-    p.is_v = 1;
-    p.n_lines = d.dst_w;
-    PassConfig c = pl->cfg_v;
-    if (p4 || out0 != 0 || out1 != d.dst_h) c = choose_generic_config(pl->v.hostdev, p.channels, out0, out1, pl->smem_optin);
-    p.lines_per_block = c.lines_per_block;
-    p.tile_out = c.tile_out;
-    p.out0 = out0;
-    p.out1 = out1;
-    p.span_a = c.span_a;
-    p.pitch = c.pitch;
-    p.src = d_mid;
-    p.src_pitch = (long long)mid_pitch(pl, d.dst_w);
-    p.src_type = AVIRB200_F32;
-    p.src_row_base = mid_row_base;
-    p.dst = d_dst;
-    p.dst_pitch = (long long)dst_pitch;
-    p.dst_type = d.out_type;
-    p.dst_row_base = out0;
-    ++*launches;
-    const int r = launch_generic(p, c, st);
-    return r != 0 ? r : finish();
+    return 0;
 }
 
 // ---- NCCL through dlopen (no link-time dependency) -------------------------------------------
@@ -1394,20 +1336,22 @@ int resize_region(const avirb200_plan* pl, const avirb200_window_info* win, int 
         kdst = out32;
         kdst_pitch = (size_t)w * d.channels;
     }
-    int r;
-    if (win == nullptr) {
-        r = run_row_pass(pl, ksrc, ksrc_pitch, static_cast<float*>(d_ws), d.src_h, st, &launches, wsb + ws.src4);
-        if (r != 0) return r;
-        r = run_col_pass(pl, static_cast<const float*>(d_ws), 0, kdst, kdst_pitch, 0, d.dst_h, st,
-                         &launches, wsb + ws.dst4);
-    } else {
-        const avs::StreamColumns cols{x0, x0 + w, win->src_x0, win->src_x0 + win->src_w};
-        r = run_row_pass(pl, ksrc, ksrc_pitch, static_cast<float*>(d_ws), src_h, st, &launches, wsb + ws.src4, 0, 0,
-                         nullptr, nullptr, &cols);
-        if (r != 0) return r;
-        r = run_col_pass(pl, static_cast<const float*>(d_ws), win->mid_row0, kdst, kdst_pitch, y0, y0 + h, st,
-                         &launches, wsb + ws.dst4, win->mid_rows, nullptr, w);
+    // (a window: the intermediate columns [x0, x0 + w) from its footprint's source columns, and the column
+    // pass over those columns only)
+    float* mid = static_cast<float*>(d_ws);
+    PassRequest row = row_request(d, ksrc, ksrc_pitch, src_h, mid, mid_pitch(pl, w));
+    const int mid_lo = win ? win->mid_row0 : 0, mid_hi = win ? win->mid_row0 + win->mid_rows : d.src_h;
+    PassRequest col = col_request(d, w, mid, mid_pitch(pl, w), mid_lo, mid_hi, kdst, kdst_pitch, y0, y0 + h);
+    if (win != nullptr) {
+        row.out0 = row.dst_base = x0;
+        row.out1 = x0 + w;
+        row.src_base = row.src_lo = win->src_x0;
+        row.src_hi = win->src_x0 + win->src_w;
     }
+    row.scratch4 = wsb + ws.src4;
+    col.scratch4 = wsb + ws.dst4;
+    int r = run_pass(pl, row, st, &launches);
+    if (r == 0) r = run_pass(pl, col, st, &launches);
     if (r == 0 && pl->io_out_type == AVIRB200_F64) {
         const int re = w * d.channels;
         const long long n = (long long)re * h;
@@ -1538,8 +1482,9 @@ int avirb200_row_pass_device(const avirb200_plan* pl, const void* d_src, size_t 
         return fail(AVIRB200_ERR_BAD_ARG, "null argument");
     if (plan_has_f64(pl)) return fail(AVIRB200_ERR_UNSUPPORTED, "per-pass entry points: no double buffers, no error diffusion");
     int launches = 0;
-    return run_row_pass(pl, d_src, src_pitch, static_cast<float*>(d_ws), pl->desc.src_h,
-                        static_cast<cudaStream_t>(stream), &launches, static_cast<char*>(d_ws) + ws_layout(pl).src4);
+    PassRequest q = row_request(pl->desc, d_src, src_pitch, pl->desc.src_h, static_cast<float*>(d_ws), mid_pitch(pl));
+    q.scratch4 = static_cast<char*>(d_ws) + ws_layout(pl).src4;
+    return run_pass(pl, q, static_cast<cudaStream_t>(stream), &launches);
 }
 
 int avirb200_col_pass_device(const avirb200_plan* pl, const void* d_ws, void* d_dst,
@@ -1547,10 +1492,12 @@ int avirb200_col_pass_device(const avirb200_plan* pl, const void* d_ws, void* d_
     if (pl == nullptr || d_dst == nullptr || d_ws == nullptr)
         return fail(AVIRB200_ERR_BAD_ARG, "null argument");
     if (plan_has_f64(pl)) return fail(AVIRB200_ERR_UNSUPPORTED, "per-pass entry points: no double buffers, no error diffusion");
+    const avirb200_plan_desc& d = pl->desc;
     int launches = 0;
-    return run_col_pass(pl, static_cast<const float*>(d_ws), 0, d_dst, dst_pitch, 0, pl->desc.dst_h,
-                        static_cast<cudaStream_t>(stream), &launches,
-                        static_cast<char*>(const_cast<void*>(d_ws)) + ws_layout(pl).dst4);
+    PassRequest q = col_request(d, d.dst_w, static_cast<const float*>(d_ws), mid_pitch(pl), 0, d.src_h, d_dst, dst_pitch,
+                                0, d.dst_h);
+    q.scratch4 = static_cast<char*>(const_cast<void*>(d_ws)) + ws_layout(pl).dst4;
+    return run_pass(pl, q, static_cast<cudaStream_t>(stream), &launches);
 }
 
 int avirb200_resize_device_batch(const avirb200_plan* pl, int n, const void* const* d_srcs, size_t src_pitch,
@@ -1704,9 +1651,10 @@ int avirb200_resize_host(avirb200_plan* pl, const void* h_src, size_t src_pitch,
         { const int r0 = copy_in(0); if (r0 != 0) return r0; }
         auto col_band = [&](int b) -> int {
             char* dd = static_cast<char*>(pl->d_dst) + (size_t)si[b].dst_row0 * out_row;
-            int r = run_col_pass(pl, static_cast<const float*>(pl->d_ws), 0, dd, ddst_pitch, si[b].dst_row0,
-                                 si[b].dst_row0 + si[b].dst_rows, pl->stream, &launches,
-                                 dst4 + (size_t)si[b].dst_row0 * dst4_row);
+            PassRequest q = col_request(d, d.dst_w, static_cast<const float*>(pl->d_ws), rowf, 0, d.src_h, dd, ddst_pitch,
+                                        si[b].dst_row0, si[b].dst_row0 + si[b].dst_rows);
+            q.scratch4 = dst4 + (size_t)si[b].dst_row0 * dst4_row;
+            const int r = run_pass(pl, q, pl->stream, &launches);
             if (r != 0) return r;
             CUDA_TRY(cudaEventRecord(pl->ev_out[b], pl->stream));
             CUDA_TRY(cudaStreamWaitEvent(pl->stream_out, pl->ev_out[b], 0));
@@ -1725,9 +1673,10 @@ int avirb200_resize_host(avirb200_plan* pl, const void* h_src, size_t src_pitch,
         for (int b = 0; b < nb; ++b) {
             if (b + 1 < nb) { const int r0 = copy_in(b + 1); if (r0 != 0) return r0; }
             CUDA_TRY(cudaStreamWaitEvent(pl->stream, pl->ev_in[b], 0));
-            int r = run_row_pass(pl, static_cast<const char*>(pl->d_src) + (size_t)si[b].src_row0 * in_row,
-                                 dsrc_pitch, static_cast<float*>(pl->d_ws) + (size_t)si[b].src_row0 * rowf,
-                                 si[b].src_rows, pl->stream, &launches, src4 + (size_t)si[b].src_row0 * src4_row);
+            PassRequest q = row_request(d, static_cast<const char*>(pl->d_src) + (size_t)si[b].src_row0 * in_row, dsrc_pitch,
+                                        si[b].src_rows, static_cast<float*>(pl->d_ws) + (size_t)si[b].src_row0 * rowf, rowf);
+            q.scratch4 = src4 + (size_t)si[b].src_row0 * src4_row;
+            int r = run_pass(pl, q, pl->stream, &launches);
             if (r != 0) return r;
             if (b > 0 && (r = col_band(b - 1)) != 0) return r; // needs rows of bands b-2 .. b only
         }
@@ -1813,11 +1762,15 @@ int avirb200_resize_sharded(const avirb200_plan* cpl, void* comm, int rank, int 
     char* dst4 = static_cast<char*>(d_ws) + ws.dst4;
     const size_t src4_row = (size_t)d.src_w * 4 * in_el;
     int launches = 0;
+    // the band's passes: its own rows into `own`, its destination rows from the intermediate rows it holds
+    PassRequest row = row_request(d, d_src, src_pitch, si.src_rows, own, rowf);
+    row.scratch4 = src4;
+    PassRequest col = col_request(d, d.dst_w, mid, rowf, si.need_row0, si.need_row0 + si.need_rows, d_dst, dst_pitch,
+                                  si.dst_row0, si.dst_row0 + si.dst_rows);
+    col.scratch4 = dst4;
     if (nranks <= 1) {
-        r = run_row_pass(pl, d_src, src_pitch, own, si.src_rows, st, &launches, src4);
-        if (r != 0) return r;
-        r = run_col_pass(pl, mid, si.need_row0, d_dst, dst_pitch, si.dst_row0, si.dst_row0 + si.dst_rows, st, &launches, dst4,
-                         si.need_rows);
+        r = run_pass(pl, row, st, &launches);
+        if (r == 0) r = run_pass(pl, col, st, &launches);
         pl->last_launches = launches;
         return r;
     }
@@ -1850,9 +1803,10 @@ int avirb200_resize_sharded(const avirb200_plan* cpl, void* comm, int rank, int 
         *hs = seq;
         const char* srcb = static_cast<const char*>(d_src);
         auto rows_pass = [&](int row0, int nrows) -> int {
-            if (nrows <= 0) return 0;
-            return run_row_pass(pl, srcb + (size_t)row0 * src_pitch * in_el, src_pitch, own + (size_t)row0 * rowf,
-                                nrows, st, &launches, src4 + (size_t)row0 * src4_row);
+            PassRequest q = row_request(d, srcb + (size_t)row0 * src_pitch * in_el, src_pitch, nrows,
+                                        own + (size_t)row0 * rowf, rowf);
+            q.scratch4 = src4 + (size_t)row0 * src4_row;
+            return run_pass(pl, q, st, &launches);
         };
         const int need_up = (link.up && si.halo_up > 0) ? 1 : 0;
         const int need_down = (link.dn && si.halo_down > 0) ? 1 : 0;
@@ -1868,41 +1822,44 @@ int avirb200_resize_sharded(const avirb200_plan* cpl, void* comm, int rank, int 
         // streaming kernel pushes with the copy engines, a column pass that is not pulls into the workspace.
         const bool fused = pl->opt_overlap == 3 && avs::stream_fused_rx_ok(link);
         const bool fused_tx = pl->opt_overlap == 3 && avs::stream_fused_tx_ok(link);
-        bool sent = false, pushed = false;
+        bool pushed = false;
         if (fused_tx && top_rows + bot_rows > 0) {
-            if ((r = run_row_pass(pl, d_src, src_pitch, own, si.src_rows, st, &launches, src4, 0, 0, &link, &sent)) != 0) return r;
+            PassRequest q = row;
+            const bool send = pass_family(pl, q).family == kFamilyStream;
+            if (send) q.link = &link;
+            if ((r = run_pass(pl, q, st, &launches)) != 0) return r;
+            if (!send) { // (not on the streaming kernel: the copy engines push)
+                if ((r = sharded_push(pl, st, own, link, hs)) != 0) return r;
+                pushed = true;
+            }
         } else {
             // 1. the rows the neighbours need (one launch on the streaming kernel: two line segments),
             // 2. their push on the exchange stream, 3. the interior rows
             // (boundary rows first only on request, AVIRB200_OPT_OVERLAP_HALO = 2: the copy-engine push
             // of cfg3's 1.2 MB is short next to the extra launch the split costs)
             const bool split = pl->opt_overlap == 2 && top_rows + bot_rows < si.src_rows;
-            if (split && !use_pad4(pl) && row_pass_on_stream(pl, d_src, src_pitch, own)) {
-                if (top_rows + bot_rows > 0 &&
-                    (r = run_row_pass(pl, d_src, src_pitch, own, si.src_rows, st, &launches, nullptr, top_rows, bot_rows)) != 0)
-                    return r;
+            if (split && !use_pad4(pl) && pass_family(pl, row).family == kFamilyStream) {
+                PassRequest q = row;
+                q.seg_top = top_rows;
+                q.seg_bot = bot_rows;
+                if (top_rows + bot_rows > 0 && (r = run_pass(pl, q, st, &launches)) != 0) return r;
             } else if (split) {
                 if ((r = rows_pass(0, top_rows)) != 0) return r;
                 if ((r = rows_pass(si.src_rows - bot_rows, bot_rows)) != 0) return r;
-            } else if ((r = rows_pass(0, si.src_rows)) != 0) {
+            } else if ((r = run_pass(pl, row, st, &launches)) != 0) {
                 return r;
             }
             if ((r = sharded_push(pl, st, own, link, hs)) != 0) return r;
-            sent = pushed = true;
-            if (split && (r = rows_pass(top_rows, si.src_rows - top_rows - bot_rows)) != 0) return r;
-        }
-        if (!sent && top_rows + bot_rows > 0) { // the fused row pass did not run on the streaming kernel
-            if ((r = sharded_push(pl, st, own, link, hs)) != 0) return r;
             pushed = true;
+            if (split && (r = rows_pass(top_rows, si.src_rows - top_rows - bot_rows)) != 0) return r;
         }
         // 4. the neighbours' rows: in place (fused), or wait for their sequence numbers and move them
         // mailbox -> workspace
-        r = 1;
-        if (fused && (need_up || need_down)) {
-            r = run_col_pass(pl, mid, si.need_row0, d_dst, dst_pitch, si.dst_row0, si.dst_row0 + si.dst_rows, st, &launches,
-                             dst4, si.need_rows, &link);
-        }
-        if (r == 1) {
+        if (fused && (need_up || need_down) && pass_family(pl, col).family == kFamilyStream) {
+            PassRequest q = col;
+            q.link = &link;
+            r = run_pass(pl, q, st, &launches);
+        } else {
             if (need_up || need_down) {
                 (void)cudaGetLastError();
                 halo_pull_kernel<<<64, 256, 0, st>>>(link.mine.flags, seq, need_up, need_down,
@@ -1914,8 +1871,7 @@ int avirb200_resize_sharded(const avirb200_plan* cpl, void* comm, int rank, int 
                 ++launches;
                 CUDA_TRY(cudaGetLastError());
             }
-            r = run_col_pass(pl, mid, si.need_row0, d_dst, dst_pitch, si.dst_row0, si.dst_row0 + si.dst_rows, st, &launches,
-                             dst4, si.need_rows);
+            r = run_pass(pl, col, st, &launches);
         }
         // the pushes read this call's workspace: the caller's stream does not end before them
         if (pushed) CUDA_TRY(cudaStreamWaitEvent(st, pl->ev_x1, 0));
@@ -1923,8 +1879,7 @@ int avirb200_resize_sharded(const avirb200_plan* cpl, void* comm, int rank, int 
         return r;
     }
     // NCCL schedule: whole row pass, send/recv group, column pass, one stream
-    r = run_row_pass(pl, d_src, src_pitch, own, si.src_rows, st, &launches, src4);
-    if (r != 0) return r;
+    if ((r = run_pass(pl, row, st, &launches)) != 0) return r;
     NCCL_TRY(nc->GroupStart());
     if (rank > 0) {
         if (top_rows > 0) NCCL_TRY(nc->Send(own, (size_t)top_rows * rowf, 7, rank - 1, comm, st));
@@ -1937,8 +1892,7 @@ int avirb200_resize_sharded(const avirb200_plan* cpl, void* comm, int rank, int 
             NCCL_TRY(nc->Recv(own + (size_t)si.src_rows * rowf, (size_t)si.halo_down * rowf, 7, rank + 1, comm, st));
     }
     NCCL_TRY(nc->GroupEnd());
-    r = run_col_pass(pl, mid, si.need_row0, d_dst, dst_pitch, si.dst_row0, si.dst_row0 + si.dst_rows, st, &launches, dst4,
-                     si.need_rows);
+    r = run_pass(pl, col, st, &launches);
     pl->last_launches = launches;
     return r;
 }
@@ -1988,8 +1942,7 @@ int avirb200_resize_sharded_local(const avirb200_plan* pl, int nranks, const voi
     const size_t in_el = elem_size(d.in_type), out_el = elem_size(d.out_type);
     std::vector<avirb200_shard_info> si(nranks);
     std::vector<float*> mid(nranks), own(nranks);
-    std::vector<const char*> src(nranks);
-    std::vector<char*> dst(nranks), src4(nranks), dst4(nranks);
+    std::vector<PassRequest> row(nranks), col(nranks);
     char* base = static_cast<char*>(d_ws);
     for (int r = 0; r < nranks; ++r) { // every band's segment: as avirb200_shard_workspace_bytes lays it out
         int e = shard_compute(pl, r, nranks, &si[r]);
@@ -1997,18 +1950,19 @@ int avirb200_resize_sharded_local(const avirb200_plan* pl, int nranks, const voi
         const WsLayout ws = ws_layout(pl, si[r]);
         mid[r] = reinterpret_cast<float*>(base);
         own[r] = mid[r] + (size_t)si[r].halo_up * rowf;
-        src4[r] = base + ws.src4;
-        dst4[r] = base + ws.dst4;
+        row[r] = row_request(d, static_cast<const char*>(d_src) + (size_t)si[r].src_row0 * src_pitch * in_el, src_pitch,
+                             si[r].src_rows, own[r], rowf);
+        row[r].scratch4 = base + ws.src4;
+        col[r] = col_request(d, d.dst_w, mid[r], rowf, si[r].need_row0, si[r].need_row0 + si[r].need_rows,
+                             static_cast<char*>(d_dst) + (size_t)si[r].dst_row0 * dst_pitch * out_el, dst_pitch,
+                             si[r].dst_row0, si[r].dst_row0 + si[r].dst_rows);
+        col[r].scratch4 = base + ws.dst4;
         base += ws.total;
-        src[r] = static_cast<const char*>(d_src) + (size_t)si[r].src_row0 * src_pitch * in_el;
-        dst[r] = static_cast<char*>(d_dst) + (size_t)si[r].dst_row0 * dst_pitch * out_el;
     }
     int launches = 0;
     // The fused halo exchange of avirb200_resize_sharded (AVIRB200_OPT_OVERLAP_HALO = 3), with every band's
     // mailbox (one slot) in this device's memory: the same two kernels, parameters and protocol as between
-    // ranks.  Only when every band may run both fused halves and both its passes run on the streaming kernel
-    // (a widened plan's kernels see its scratch copies).
-    const bool p4 = use_pad4(pl);
+    // ranks.  Only when every band may run both fused halves and both its passes run on the streaming kernel.
     std::vector<avs::StreamLink> link(nranks);
     std::vector<MailboxLayout> box(nranks);
     std::vector<size_t> box_off(nranks + 1, 0);
@@ -2017,9 +1971,8 @@ int avirb200_resize_sharded_local(const avirb200_plan* pl, int nranks, const voi
         link[r].me = &si[r];
         if (r > 0) link[r].up = &si[r - 1];
         if (r + 1 < nranks) link[r].dn = &si[r + 1];
-        fused = avs::stream_fused_tx_ok(link[r]) &&
-                row_pass_on_stream(pl, p4 ? src4[r] : src[r], p4 ? (size_t)d.src_w * 4 : src_pitch, own[r]) &&
-                col_pass_on_stream(pl, p4 ? dst4[r] : dst[r], p4 ? (size_t)d.dst_w * 4 : dst_pitch, mid[r]);
+        fused = avs::stream_fused_tx_ok(link[r]) && pass_family(pl, row[r]).family == kFamilyStream &&
+                pass_family(pl, col[r]).family == kFamilyStream;
         box[r] = MailboxLayout(pl, si[r]);
         box_off[r + 1] = box_off[r] + box[r].bytes(1);
     }
@@ -2036,25 +1989,17 @@ int avirb200_resize_sharded_local(const avirb200_plan* pl, int nranks, const voi
         for (int r = 0; r < nranks; ++r) {
             if (r > 0) link[r].above = link[r - 1].mine;
             if (r + 1 < nranks) link[r].below = link[r + 1].mine;
+            if (avs::stream_rows_up(link[r]) + avs::stream_rows_down(link[r]) > 0) row[r].link = &link[r];
+            col[r].link = &link[r];
         }
-        for (int r = 0; r < nranks && e == 0; ++r) {
-            const bool tx = avs::stream_rows_up(link[r]) + avs::stream_rows_down(link[r]) > 0;
-            bool sent = false;
-            e = run_row_pass(pl, src[r], src_pitch, own[r], si[r].src_rows, st, &launches, src4[r], 0, 0,
-                             tx ? &link[r] : nullptr, &sent);
-            if (e == 0 && tx && !sent) e = fail(AVIRB200_ERR_CUDA, "sharded_local: the streaming row pass did not take the band");
-        }
-        for (int r = 0; r < nranks && e == 0; ++r) {
-            e = run_col_pass(pl, mid[r], si[r].need_row0, dst[r], dst_pitch, si[r].dst_row0, si[r].dst_row0 + si[r].dst_rows,
-                             st, &launches, dst4[r], si[r].need_rows, &link[r]);
-            if (e == 1) e = fail(AVIRB200_ERR_CUDA, "sharded_local: the streaming column pass did not take the band");
-        }
+        for (int r = 0; r < nranks && e == 0; ++r) e = run_pass(pl, row[r], st, &launches);
+        for (int r = 0; r < nranks && e == 0; ++r) e = run_pass(pl, col[r], st, &launches);
         cudaFreeAsync(boxes, st);
         pl->last_launches = launches;
         return e;
     }
     for (int r = 0; r < nranks; ++r) { // every band's row pass
-        int e = run_row_pass(pl, src[r], src_pitch, own[r], si[r].src_rows, st, &launches, src4[r]);
+        int e = run_pass(pl, row[r], st, &launches);
         if (e != 0) return e;
     }
     for (int r = 0; r < nranks; ++r) { // the "exchange"
@@ -2069,8 +2014,7 @@ int avirb200_resize_sharded_local(const avirb200_plan* pl, int nranks, const voi
         }
     }
     for (int r = 0; r < nranks; ++r) {
-        int e = run_col_pass(pl, mid[r], si[r].need_row0, dst[r], dst_pitch, si[r].dst_row0,
-                             si[r].dst_row0 + si[r].dst_rows, st, &launches, dst4[r], si[r].need_rows);
+        int e = run_pass(pl, col[r], st, &launches);
         if (e != 0) return e;
     }
     pl->last_launches = launches;

@@ -271,19 +271,6 @@ inline void fast_plan_free(FastPlan& f) {
     f.h.arena = f.v.arena = nullptr;
 }
 
-inline void fast_fill_common(FastParams& p, const avirb200_plan_desc& d, const float* lut) {
-    p.gamma_in = (d.use_gamma & 1) ? 1 : 0;
-    p.gamma_out = (d.use_gamma & 2) ? 1 : 0;
-    p.alpha_index = d.alpha_index;
-    p.in_gamma_mult = d.in_gamma_mult;
-    p.out_gamma_mult = d.out_gamma_mult;
-    p.srgb_lut = lut;
-    p.round_mode = d.round_mode;
-    p.tr_mul = d.tr_mul;
-    p.tr_mul_inv = d.tr_mul_inv;
-    p.pk_out = d.pk_out;
-}
-
 // Persistent launch: kFastBlocksPerSM blocks per SM of the plan's device (or fewer when there are fewer tiles).
 inline int fast_launch(const FastParams& p, size_t smem, int sum_mode, int sm_count, cudaStream_t st) {
     const long long tiles = (long long)((p.out1 - p.out0 + p.tile_out - 1) / p.tile_out) *
@@ -315,8 +302,8 @@ inline int fast_launch(const FastParams& p, size_t smem, int sum_mode, int sm_co
         launched = true;                                                                           \
     }
     bool launched = false;
-    const bool plain_f32 = (p.dst_type == AVIRB200_F32 && !p.gamma_out);
-    const bool int_plain = (p.dst_type != AVIRB200_F32 && !p.gamma_out && p.tr_mul == 1.0f); // integer destination, no output gamma, no truncation
+    const bool plain_f32 = (p.dst_type == AVIRB200_F32 && !p.px.gamma_out);
+    const bool int_plain = (p.dst_type != AVIRB200_F32 && !p.px.gamma_out && p.px.tr_mul == 1.0f); // integer destination, no output gamma, no truncation
     AVB_TRY(AVIRB200_SUM_DIL8, 2, kVarResizeDil24D2, kVarFirDil8R1, -1, 0)        // cfg3 (float8_dil)
     AVB_TRY(AVIRB200_SUM_DIL8, 2, kVarResizeDil56D4, kVarFirDil8R1, -1, -1)       // cfg5
     AVB_TRY(AVIRB200_SUM_INL, 3, kVarFirInl7R1, kVarResizeInl18D2, kVarFirInl7R1, 1)   // cfg3 (float4)
@@ -403,70 +390,34 @@ inline void fast_set_footprint(FastParams& p, const FastFootprint& f) {
     p.taps_floats = f.taps_floats;
 }
 
-// Returns 0 = launched, -2 = not applicable (alignment: the caller runs the generic kernel),
-// -1 = launch error.
-// mid_pitch: floats between intermediate rows.
-// A window: intermediate columns [out0, out1) (stored from the intermediate's column 0 on) from a source
-// buffer whose column 0 is source column src_col0; out1 < 0: every column of the whole line.
-inline int fast_row_pass(const FastPlan& f, const avirb200_plan_desc& d, const void* d_src, size_t src_pitch,
-                         float* d_mid, size_t mid_pitch, int rows, const float* lut, int sm_count, cudaStream_t st,
-                         int out0 = 0, int out1 = -1, int src_col0 = 0) {
-    const size_t es = elem_size(d.in_type);
-    if (((uintptr_t)d_src % (4 * es)) != 0 || (src_pitch % 4) != 0 || ((uintptr_t)d_mid % 16) != 0)
-        return -2;
-    if (out1 < 0) out1 = d.dst_w;
-    FastParams p;
-    memset(&p, 0, sizeof p);
-    fast_fill_common(p, d, lut);
-    p.ax = f.h.ax;
-    p.is_v = 0;
-    p.n_lines = rows;
-    FastFootprint fpnt = f.h.fpnt;
-    if (out0 != 0 || out1 != d.dst_w) { // a window: footprint of its own tiles
-        fpnt = fast_footprint_all(f.h.hax, f.h.tile_out, out0, out1, f.h.raw);
-        if (fpnt.smem > kFastSmemBudget) return -2;
-    }
-    p.tile_out = f.h.tile_out;
-    p.out0 = out0; p.out1 = out1;
-    fast_set_footprint(p, fpnt);
-    fast_set_const_taps(p, f.h);
-    p.tile_ranges = fast_tile_table(f.h, out0, out1);
-    if (p.tile_ranges == nullptr) return -1;
-    p.src = d_src; p.src_pitch = (long long)src_pitch; p.src_type = d.in_type;
-    p.src_row_base = src_col0;
-    p.dst = d_mid; p.dst_pitch = (long long)mid_pitch; p.dst_type = AVIRB200_F32;
-    p.dst_row_base = out0;
-    return fast_launch(p, fpnt.smem, d.sum_mode, sm_count, st);
+// The footprint of the tiles of the final outputs [out0, out1): the plan's own for the whole line, else
+// that range's own tiles' (a window's columns, a band's rows; it may exceed kFastSmemBudget).
+inline FastFootprint fast_range_footprint(const FastPass& fp, int out0, int out1) {
+    if (out0 == 0 && out1 == fp.hax.dst_len) return fp.fpnt;
+    return fast_footprint_all(fp.hax, fp.tile_out, out0, out1, fp.raw);
 }
 
-inline int fast_col_pass(const FastPlan& f, const avirb200_plan_desc& d, const float* d_mid, size_t mid_pitch,
-                         int mid_row_base, void* d_dst, size_t dst_pitch, int out0, int out1,
-                         const float* lut, int sm_count, cudaStream_t st) {
-    const size_t es = elem_size(d.out_type);
-    if (((uintptr_t)d_dst % (2 * es)) != 0 || (dst_pitch % 2) != 0 || ((uintptr_t)d_mid % 16) != 0)
-        return -2;
+// Launches the pass q (its buffers as the kernel sees them) with the footprint fast_range_footprint gave.
+// Returns 0 = launched, -1 = launch error, -2 = more tiles than a launch can count.
+inline int fast_pass(const FastPass& fp, const PassRequest& q, const FastFootprint& fpnt, const PixelStage& px,
+                     int sum_mode, int sm_count, cudaStream_t st) {
     FastParams p;
     memset(&p, 0, sizeof p);
-    fast_fill_common(p, d, lut);
-    p.ax = f.v.ax;
-    p.is_v = 1;
-    p.n_lines = d.dst_w;
-    FastFootprint fpnt = f.v.fpnt;
-    if (out0 != 0 || out1 != d.dst_h) { // a shard: footprint of its own tiles
-        fpnt = fast_footprint_all(f.v.hax, f.v.tile_out, out0, out1);
-        if (fpnt.smem > 220 * 1024) return -2;
-    }
-    p.tile_out = f.v.tile_out;
-    p.out0 = out0; p.out1 = out1;
+    p.ax = fp.ax;
+    p.is_v = q.is_v ? 1 : 0;
+    p.n_lines = q.lines;
+    p.tile_out = fp.tile_out;
+    p.out0 = q.out0; p.out1 = q.out1;
     fast_set_footprint(p, fpnt);
-    fast_set_const_taps(p, f.v);
-    p.tile_ranges = fast_tile_table(f.v, out0, out1);
+    fast_set_const_taps(p, fp);
+    p.tile_ranges = fast_tile_table(fp, q.out0, q.out1);
     if (p.tile_ranges == nullptr) return -1;
-    p.src = d_mid; p.src_pitch = (long long)mid_pitch; p.src_type = AVIRB200_F32;
-    p.src_row_base = mid_row_base;
-    p.dst = d_dst; p.dst_pitch = (long long)dst_pitch; p.dst_type = d.out_type;
-    p.dst_row_base = out0;
-    return fast_launch(p, fpnt.smem, d.sum_mode, sm_count, st);
+    p.src = q.src; p.src_pitch = (long long)q.src_pitch; p.src_type = q.src_type;
+    p.src_row_base = q.src_base;
+    p.dst = q.dst; p.dst_pitch = (long long)q.dst_pitch; p.dst_type = q.dst_type;
+    p.dst_row_base = q.dst_base;
+    p.px = px;
+    return fast_launch(p, fpnt.smem, sum_mode, sm_count, st);
 }
 
 } // namespace avb

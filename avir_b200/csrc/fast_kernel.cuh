@@ -95,11 +95,7 @@ struct FastParams {
     long long dst_pitch;
     int dst_type;
     int dst_row_base;     // final output stored at the destination's position 0 (column pass: row; row pass: column)
-    int gamma_in, gamma_out, alpha_index;
-    float in_gamma_mult, out_gamma_mult;
-    const float* srgb_lut;
-    int round_mode;
-    float tr_mul, tr_mul_inv, pk_out;
+    PixelStage px;
 };
 
 // ---- host+device range arithmetic (unclamped: tiles materialise edge replicas) ----------------
@@ -157,16 +153,16 @@ __device__ __forceinline__ void cp_async_wait_all() {
 
 // Integer destinations: round (the class's own round()), clamp (avir.h:4392-4419).
 __device__ __forceinline__ float epilogue_round_c4(const FastParams& p, float v) {
-    if (p.tr_mul == 1.0f) v = round_out(v, p.round_mode);
-    else v = __fmul_rn(round_out(__fmul_rn(v, p.tr_mul_inv), p.round_mode), p.tr_mul);
-    return v < 0.0f ? 0.0f : (v > p.pk_out ? p.pk_out : v);
+    if (p.px.tr_mul == 1.0f) v = round_out(v, p.px.round_mode);
+    else v = __fmul_rn(round_out(__fmul_rn(v, p.px.tr_mul_inv), p.px.round_mode), p.px.tr_mul);
+    return v < 0.0f ? 0.0f : (v > p.px.pk_out ? p.px.pk_out : v);
 }
 
 // Output stage for one element (gamma -> round -> clamp), 4-channel images.
 __device__ __forceinline__ float epilogue_value_c4(const FastParams& p, float v, int c) {
-    if (p.gamma_out) {
-        if (c == p.alpha_index) v = __fmul_rn(v, p.out_gamma_mult);
-        else v = __fmul_rn(lin2srgb(v), p.out_gamma_mult);
+    if (p.px.gamma_out) {
+        if (c == p.px.alpha_index) v = __fmul_rn(v, p.px.out_gamma_mult);
+        else v = __fmul_rn(lin2srgb(v), p.px.out_gamma_mult);
     }
     if (p.dst_type != AVIRB200_F32) v = epilogue_round_c4(p, v);
     return v;
@@ -410,9 +406,9 @@ __device__ __forceinline__ void sink_store(const FastParams& p, const Sink& k, i
         unsigned char* g2 = k.gp + (size_t)(j - k.grow_base) * k.grow;
         // (no bit-depth truncation, fast_launch(): one rounding conversion per sample, clamp and
         // narrow in integers, selects and predicated stores instead of branches)
-        const int pk = (int)p.pk_out;
-        const int a = imin(imax(round_out_int(v.x, p.round_mode), 0), pk);
-        const int b = imin(imax(round_out_int(v.y, p.round_mode), 0), pk);
+        const int pk = (int)p.px.pk_out;
+        const int a = imin(imax(round_out_int(v.x, p.px.round_mode), 0), pk);
+        const int b = imin(imax(round_out_int(v.y, p.px.round_mode), 0), pk);
         const bool narrow = (p.dst_type == AVIRB200_U8);
         if (narrow) *reinterpret_cast<unsigned short*>(g2) = (unsigned short)(a | (b << 8));
         if (!narrow) *reinterpret_cast<unsigned*>(g2) = (unsigned)a | ((unsigned)b << 16);
@@ -599,22 +595,22 @@ __device__ __forceinline__ void stage_source(const FastParams& p, float2* buf, c
                 if (p.src_type == AVIRB200_U8) {
                     const uchar4 b = __ldg(reinterpret_cast<const uchar4*>(static_cast<const unsigned char*>(p.src) + rowoff) + x);
                     v = make_float4((float)b.x, (float)b.y, (float)b.z, (float)b.w);
-                    if (p.gamma_in) {
-                        const int ai = p.alpha_index;
-                        v.x = (ai == 0) ? __fmul_rn(v.x, p.in_gamma_mult) : p.srgb_lut[b.x];
-                        v.y = p.srgb_lut[b.y];
-                        v.z = p.srgb_lut[b.z];
-                        v.w = (ai == 3) ? __fmul_rn(v.w, p.in_gamma_mult) : p.srgb_lut[b.w];
+                    if (p.px.gamma_in) {
+                        const int ai = p.px.alpha_index;
+                        v.x = (ai == 0) ? __fmul_rn(v.x, p.px.in_gamma_mult) : p.px.srgb_lut[b.x];
+                        v.y = p.px.srgb_lut[b.y];
+                        v.z = p.px.srgb_lut[b.z];
+                        v.w = (ai == 3) ? __fmul_rn(v.w, p.px.in_gamma_mult) : p.px.srgb_lut[b.w];
                     }
                 } else {
                     const ushort4 b = __ldg(reinterpret_cast<const ushort4*>(static_cast<const unsigned short*>(p.src) + rowoff) + x);
                     v = make_float4((float)b.x, (float)b.y, (float)b.z, (float)b.w);
-                    if (p.gamma_in) {
-                        const int ai = p.alpha_index;
-                        v.x = (ai == 0) ? __fmul_rn(v.x, p.in_gamma_mult) : srgb2lin(v.x, p.in_gamma_mult);
-                        v.y = srgb2lin(v.y, p.in_gamma_mult);
-                        v.z = srgb2lin(v.z, p.in_gamma_mult);
-                        v.w = (ai == 3) ? __fmul_rn(v.w, p.in_gamma_mult) : srgb2lin(v.w, p.in_gamma_mult);
+                    if (p.px.gamma_in) {
+                        const int ai = p.px.alpha_index;
+                        v.x = (ai == 0) ? __fmul_rn(v.x, p.px.in_gamma_mult) : srgb2lin(v.x, p.px.in_gamma_mult);
+                        v.y = srgb2lin(v.y, p.px.in_gamma_mult);
+                        v.z = srgb2lin(v.z, p.px.in_gamma_mult);
+                        v.w = (ai == 3) ? __fmul_rn(v.w, p.px.in_gamma_mult) : srgb2lin(v.w, p.px.in_gamma_mult);
                     }
                 }
                 *reinterpret_cast<float4*>(buf + pos * kFastPitch + r * 2) = v;
@@ -658,22 +654,22 @@ __device__ __forceinline__ void convert_raw(const FastParams& p, const unsigned 
         if (p.src_type == AVIRB200_U8) {
             const uchar4 b = reinterpret_cast<const uchar4*>(raw)[idx];
             v = make_float4((float)b.x, (float)b.y, (float)b.z, (float)b.w);
-            if (p.gamma_in) {
-                const int ai = p.alpha_index;
-                v.x = (ai == 0) ? __fmul_rn(v.x, p.in_gamma_mult) : lut[b.x];
+            if (p.px.gamma_in) {
+                const int ai = p.px.alpha_index;
+                v.x = (ai == 0) ? __fmul_rn(v.x, p.px.in_gamma_mult) : lut[b.x];
                 v.y = lut[b.y];
                 v.z = lut[b.z];
-                v.w = (ai == 3) ? __fmul_rn(v.w, p.in_gamma_mult) : lut[b.w];
+                v.w = (ai == 3) ? __fmul_rn(v.w, p.px.in_gamma_mult) : lut[b.w];
             }
         } else {
             const ushort4 b = reinterpret_cast<const ushort4*>(raw)[idx];
             v = make_float4((float)b.x, (float)b.y, (float)b.z, (float)b.w);
-            if (p.gamma_in) {
-                const int ai = p.alpha_index;
-                v.x = (ai == 0) ? __fmul_rn(v.x, p.in_gamma_mult) : srgb2lin(v.x, p.in_gamma_mult);
-                v.y = srgb2lin(v.y, p.in_gamma_mult);
-                v.z = srgb2lin(v.z, p.in_gamma_mult);
-                v.w = (ai == 3) ? __fmul_rn(v.w, p.in_gamma_mult) : srgb2lin(v.w, p.in_gamma_mult);
+            if (p.px.gamma_in) {
+                const int ai = p.px.alpha_index;
+                v.x = (ai == 0) ? __fmul_rn(v.x, p.px.in_gamma_mult) : srgb2lin(v.x, p.px.in_gamma_mult);
+                v.y = srgb2lin(v.y, p.px.in_gamma_mult);
+                v.z = srgb2lin(v.z, p.px.in_gamma_mult);
+                v.w = (ai == 3) ? __fmul_rn(v.w, p.px.in_gamma_mult) : srgb2lin(v.w, p.px.in_gamma_mult);
             }
         }
         *reinterpret_cast<float4*>(buf + pos * kFastPitch + r * 2) = v;
@@ -738,8 +734,8 @@ fast_pass_kernel(const __grid_constant__ FastParams p) {
             for (int q = tid; q < s.ntaps_pad; q += kFastThreads) st[q] = __ldg(s.taps + q);
         }
     }
-    if (raw_src && p.gamma_in && p.src_type == AVIRB200_U8)
-        for (int q = tid; q < 256; q += kFastThreads) slut[q] = __ldg(p.srgb_lut + q);
+    if (raw_src && p.px.gamma_in && p.src_type == AVIRB200_U8)
+        for (int q = tid; q < 256; q += kFastThreads) slut[q] = __ldg(p.px.srgb_lut + q);
     // records of the first two tiles
     if (tid < kTileRec) {
         srec[0][tid] = __ldg(p.tile_ranges + (size_t)(t % tiles_x) * kTileRec + tid);

@@ -14,6 +14,7 @@
 
 #include "fast_kernel.cuh"
 #include "host_util.h"
+#include "pass_request.h"
 
 namespace avb {
 

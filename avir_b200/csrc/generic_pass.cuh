@@ -47,23 +47,18 @@ struct PassParams {
     long long dst_pitch;
     int dst_type;
     int dst_row_base;     // global output stored at the destination's position 0 (column pass: row; row pass: column)
-    // prologue / epilogue
-    int gamma_in, gamma_out, alpha_index;
-    float in_gamma_mult, out_gamma_mult;
-    const float* srgb_lut; // 256 floats (u8 input)
-    int round_mode;
-    float tr_mul, tr_mul_inv, pk_out;
+    PixelStage px;        // prologue / epilogue
 };
 
 __device__ __forceinline__ float epilogue_value(const PassParams& p, float v, int c) {
-    if (p.gamma_out) {
-        if (p.channels == 4 && c == p.alpha_index) v = __fmul_rn(v, p.out_gamma_mult);
-        else v = __fmul_rn(lin2srgb(v), p.out_gamma_mult);
+    if (p.px.gamma_out) {
+        if (p.channels == 4 && c == p.px.alpha_index) v = __fmul_rn(v, p.px.out_gamma_mult);
+        else v = __fmul_rn(lin2srgb(v), p.px.out_gamma_mult);
     }
     if (p.dst_type != AVIRB200_F32) {
-        if (p.tr_mul == 1.0f) v = round_out(v, p.round_mode);
-        else v = __fmul_rn(round_out(__fmul_rn(v, p.tr_mul_inv), p.round_mode), p.tr_mul);
-        v = v < 0.0f ? 0.0f : (v > p.pk_out ? p.pk_out : v);
+        if (p.px.tr_mul == 1.0f) v = round_out(v, p.px.round_mode);
+        else v = __fmul_rn(round_out(__fmul_rn(v, p.px.tr_mul_inv), p.px.round_mode), p.px.tr_mul);
+        v = v < 0.0f ? 0.0f : (v > p.px.pk_out ? p.px.pk_out : v);
     }
     return v;
 }
@@ -72,16 +67,16 @@ __device__ __forceinline__ float load_source(const PassParams& p, long long idx,
     float raw;
     if (p.src_type == AVIRB200_U8) {
         const unsigned char b = ((const unsigned char*)p.src)[idx];
-        if (p.gamma_in && !(p.channels == 4 && c == p.alpha_index)) return p.srgb_lut[b];
+        if (p.px.gamma_in && !(p.channels == 4 && c == p.px.alpha_index)) return p.px.srgb_lut[b];
         raw = (float)b;
     } else if (p.src_type == AVIRB200_U16) {
         raw = (float)((const unsigned short*)p.src)[idx];
     } else {
         raw = ((const float*)p.src)[idx];
     }
-    if (!p.gamma_in) return raw;
-    if (p.channels == 4 && c == p.alpha_index) return __fmul_rn(raw, p.in_gamma_mult);
-    return srgb2lin(raw, p.in_gamma_mult);
+    if (!p.px.gamma_in) return raw;
+    if (p.channels == 4 && c == p.px.alpha_index) return __fmul_rn(raw, p.px.in_gamma_mult);
+    return srgb2lin(raw, p.px.in_gamma_mult);
 }
 
 // ---- one output sample of one step ----------------------------------------------------------

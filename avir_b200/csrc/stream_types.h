@@ -9,6 +9,8 @@
 #include <string.h>
 
 #include "avirb200.h"
+#include "device_plan.h"
+#include "pass_request.h"
 
 namespace avs {
 
@@ -61,6 +63,7 @@ struct StreamParams {
     long long dst_pitch;
     int dst_type;
     int dst_row_base;     // final output stored at the destination's position 0 (row, or row-pass column)
+    // the pixel stage (avb::PixelStage) in the order the kernel's parameter space has always held it
     int gamma_out, alpha_index;
     float out_gamma_mult;
     int round_mode;
@@ -264,85 +267,6 @@ inline int stream_row_source_code(const avirb200_plan_desc& d) {
     return (d.use_gamma & 1) ? kSrcU8Srgb : d.in_type;
 }
 
-// Kernel parameters of one pass without its buffers (stream_fill_row_params / _col_params add them).
-inline void stream_fill_params(StreamParams& p, const StreamAxisPlan& ap, const avirb200_plan_desc& d) {
-    memset(&p, 0, sizeof p);
-    for (int i = 0; i < ap.nsteps; ++i) p.s[i] = ap.s[i];
-    p.src_len = ap.src_len;
-    p.src_lo = 0;
-    p.src_hi = ap.src_len;
-    p.src_type = AVIRB200_F32;
-    p.in_gamma_mult = d.in_gamma_mult;
-    p.gamma_out = (d.use_gamma & 2) ? 1 : 0;
-    p.alpha_index = d.alpha_index;
-    p.out_gamma_mult = d.out_gamma_mult;
-    p.round_mode = d.round_mode;
-    p.tr_mul = d.tr_mul;
-    p.tr_mul_inv = d.tr_mul_inv;
-    p.pk_out = d.pk_out;
-}
-
-// Output columns of a row pass and the source columns its buffer holds: intermediate columns
-// [out0, out1) (stored from the intermediate's column 0 on) from a source buffer whose column 0 is
-// source column src_lo and that holds columns [src_lo, src_hi).  The whole line: {0, dst_w, 0, src_w}.
-struct StreamColumns {
-    int out0, out1, src_lo, src_hi;
-};
-
-// Row pass: every output column of `rows` source rows from `src` into the intermediate rows at `mid`
-// (pitches in elements).  seg_top / seg_bot: only the first seg_top and the last seg_bot of those rows,
-// in one launch (seg_bot > 0: two line segments).  cols: only those columns (a window), else all.
-inline void stream_fill_row_params(StreamParams& p, const StreamAxisPlan& ap, const avirb200_plan_desc& d,
-                                   const void* src, long long src_pitch, float* mid, long long mid_pitch, int rows,
-                                   const float* lut, int seg_top = 0, int seg_bot = 0,
-                                   const StreamColumns* cols = nullptr) {
-    stream_fill_params(p, ap, d);
-    p.n_lines = rows;
-    if (seg_bot > 0) {
-        p.seg_a = seg_top;
-        p.seg_b = seg_bot;
-        p.seg_b_line0 = rows - seg_bot;
-    } else if (seg_top > 0) {
-        p.n_lines = seg_top;
-    }
-    p.out0 = 0;
-    p.out1 = d.dst_w;
-    if (cols != nullptr) {
-        p.out0 = cols->out0;
-        p.out1 = cols->out1;
-        p.dst_row_base = cols->out0;
-        p.src_lo = p.src_row_base = cols->src_lo;
-        p.src_hi = cols->src_hi;
-    }
-    p.src = src;
-    p.src_type = stream_row_source_code(d);
-    p.srgb_lut = lut;
-    p.src_pitch = src_pitch;
-    p.dst = mid;
-    p.dst_pitch = mid_pitch;
-    p.dst_type = AVIRB200_F32;
-}
-
-// Column pass: destination rows [out0, out1) into `dst` (its row 0 = row out0) from the intermediate rows
-// [mid_lo, mid_hi) the buffer at `mid` holds (its row 0 = row mid_lo).
-inline void stream_fill_col_params(StreamParams& p, const StreamAxisPlan& ap, const avirb200_plan_desc& d,
-                                   const float* mid, long long mid_pitch, int mid_lo, int mid_hi, void* dst,
-                                   long long dst_pitch, int out0, int out1) {
-    stream_fill_params(p, ap, d);
-    p.n_lines = d.dst_w;
-    p.out0 = out0;
-    p.out1 = out1;
-    p.src = mid;
-    p.src_pitch = mid_pitch;
-    p.src_row_base = mid_lo;
-    p.src_lo = mid_lo;
-    p.src_hi = mid_hi;
-    p.dst = dst;
-    p.dst_pitch = dst_pitch;
-    p.dst_type = d.out_type;
-    p.dst_row_base = out0;
-}
-
 // ---- fused halo exchange of sharded calls (StreamParams xs_* / xr_*) --------------------------------
 // A band's mailbox as the kernels see it: the rows received from the band above and from the band below,
 // the two flags (flags[0]: the rows from above are in, flags[1]: the rows from below) and the two
@@ -409,6 +333,78 @@ inline void stream_set_receiver(StreamParams& p, const StreamLink& l) {
     p.xr_seq = l.seq;
     p.xr_own_lo = l.me->src_row0;
     p.xr_own_hi = l.me->src_row0 + l.me->src_rows;
+}
+
+// Kernel parameters of the pass `q` (its buffers as the kernel sees them) on the axis plan `ap`.
+inline void stream_params(StreamParams& p, const StreamAxisPlan& ap, const avirb200_plan_desc& d,
+                          const avb::PassRequest& q, const float* lut) {
+    memset(&p, 0, sizeof p);
+    for (int i = 0; i < ap.nsteps; ++i) p.s[i] = ap.s[i];
+    p.n_lines = q.lines;
+    if (q.seg_bot > 0) {
+        p.seg_a = q.seg_top;
+        p.seg_b = q.seg_bot;
+        p.seg_b_line0 = q.lines - q.seg_bot;
+    } else if (q.seg_top > 0) {
+        p.n_lines = q.seg_top;
+    }
+    p.src_len = ap.src_len;
+    p.out0 = q.out0;
+    p.out1 = q.out1;
+    p.src = q.src;
+    p.src_type = q.is_v ? AVIRB200_F32 : stream_row_source_code(d);
+    p.src_pitch = (long long)q.src_pitch;
+    p.src_row_base = q.src_base;
+    p.src_lo = q.src_lo;
+    p.src_hi = q.src_hi;
+    p.dst = q.dst;
+    p.dst_pitch = (long long)q.dst_pitch;
+    p.dst_type = q.dst_type;
+    p.dst_row_base = q.dst_base;
+    const avb::PixelStage px = avb::pixel_stage(d, lut);
+    p.srgb_lut = px.srgb_lut;
+    p.in_gamma_mult = px.in_gamma_mult;
+    p.gamma_out = px.gamma_out;
+    p.alpha_index = px.alpha_index;
+    p.out_gamma_mult = px.out_gamma_mult;
+    p.round_mode = px.round_mode;
+    p.tr_mul = px.tr_mul;
+    p.tr_mul_inv = px.tr_mul_inv;
+    p.pk_out = px.pk_out;
+    if (q.link != nullptr) {
+        if (q.is_v) stream_set_receiver(p, *q.link);
+        else stream_set_sender(p, *q.link);
+    }
+}
+
+// The CPU emulation's entry points (tests/emul): a row pass of `rows` whole source lines (seg_top / seg_bot:
+// only its first and last lines, one launch; cols: only the intermediate columns [out0, out1) from a buffer
+// holding source columns [src_lo, src_hi)), and a column pass over d.dst_w intermediate columns.  Both are
+// requests for stream_params.
+struct StreamColumns {
+    int out0, out1, src_lo, src_hi;
+};
+inline void stream_fill_row_params(StreamParams& p, const StreamAxisPlan& ap, const avirb200_plan_desc& d,
+                                   const void* src, long long src_pitch, float* mid, long long mid_pitch, int rows,
+                                   const float* lut, int seg_top = 0, int seg_bot = 0,
+                                   const StreamColumns* cols = nullptr) {
+    avb::PassRequest q = avb::row_request(d, src, (size_t)src_pitch, rows, mid, (size_t)mid_pitch);
+    q.seg_top = seg_top;
+    q.seg_bot = seg_bot;
+    if (cols != nullptr) {
+        q.out0 = q.dst_base = cols->out0;
+        q.out1 = cols->out1;
+        q.src_base = q.src_lo = cols->src_lo;
+        q.src_hi = cols->src_hi;
+    }
+    stream_params(p, ap, d, q, lut);
+}
+inline void stream_fill_col_params(StreamParams& p, const StreamAxisPlan& ap, const avirb200_plan_desc& d,
+                                   const float* mid, long long mid_pitch, int mid_lo, int mid_hi, void* dst,
+                                   long long dst_pitch, int out0, int out1) {
+    stream_params(p, ap, d,
+                  avb::col_request(d, d.dst_w, mid, (size_t)mid_pitch, mid_lo, mid_hi, dst, (size_t)dst_pitch, out0, out1),
+                  nullptr);
 }
 
 } // namespace avs

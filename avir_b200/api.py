@@ -87,6 +87,9 @@ def host_lib():
         h.lancirb200_host_desc_get.restype = C.c_void_p
         h.lancirb200_host_desc_get.argtypes = [C.c_void_p]
         h.lancirb200_host_desc_free.argtypes = [C.c_void_p]
+        h.lancirb200_host_window.restype = C.c_int
+        h.lancirb200_host_window.argtypes = ([C.c_int] + h.lancirb200_host_resize.argtypes + [C.c_int] * 4 +
+                                             [C.c_void_p] * 4)
         _host = h
     return _host
 
@@ -272,3 +275,62 @@ class CLancIR:
                                               dst.ctypes.data, NewWidth, NewHeight, ch, p.SrcSSize,
                                               p.NewSSize, p.kx, p.ky, p.ox, p.oy, p.la)
         return r, dst
+
+    @staticmethod
+    def _window(op, src, src_shape, in_dtype, dst, NewWidth, NewHeight, out_dtype, win, p, d_workspace=None,
+                stream=0):
+        sh, sw, ch = src_shape
+        in_dtype, out_dtype = np.dtype(in_dtype), np.dtype(out_dtype)
+        if in_dtype not in _LT or out_dtype not in _LT:
+            raise AvirB200Error("CLancIR: uint8 / uint16 / float32 buffers only")
+        info, nbytes = (C.c_int * 4)(), C.c_longlong(0)
+        r = host_lib().lancirb200_host_window(op, _T[in_dtype], _T[out_dtype], src, sw, sh, dst, NewWidth, NewHeight,
+                                              ch, p.SrcSSize, p.NewSSize, p.kx, p.ky, p.ox, p.oy, p.la, *win,
+                                              d_workspace, stream, info, C.byref(nbytes))
+        return r, list(info), nbytes.value
+
+    def resizeImageWindow(self, SrcBuf, NewWidth, NewHeight, WinX, WinY, WinWidth, WinHeight, aParams=None,
+                          out_dtype=None, NewBuf=None):
+        """The destination window (WinX, WinY, WinWidth, WinHeight) of resizeImage(SrcBuf, NewWidth, NewHeight,
+        aParams) (GPU extension): SrcBuf is the whole source, the result an (WinHeight, WinWidth, C) array.
+        aParams.SrcSSize / NewSSize as in resizeImage (NewSSize: the window's scanline size).  Returns
+        (WinHeight or 0, window)."""
+        p = aParams or CLancIRParams()
+        src = _scanlines(SrcBuf, p.SrcSSize, "CLancIR.resizeImageWindow (SrcSSize)")
+        ch = src.shape[2]
+        out_dtype = np.dtype(out_dtype or (NewBuf.dtype if NewBuf is not None else src.dtype))
+        shape = (max(WinHeight, 0), max(WinWidth, 0), ch)
+        if NewBuf is None:
+            if p.NewSSize > 0:
+                raise AvirB200Error("CLancIR.resizeImageWindow: NewSSize needs a caller-supplied NewBuf")
+            dst = np.empty(shape, out_dtype)
+        else:
+            dst = NewBuf
+            if dst.shape != shape or dst.dtype != out_dtype:
+                raise AvirB200Error("CLancIR.resizeImageWindow: NewBuf is not (WinHeight, WinWidth, C) of out_dtype")
+            if p.NewSSize > 0:
+                _scanlines(dst, p.NewSSize, "CLancIR.resizeImageWindow (NewSSize)")
+            elif not dst.flags.c_contiguous:
+                raise AvirB200Error("CLancIR.resizeImageWindow: NewBuf must be contiguous without NewSSize")
+        r, _, _ = self._window(0, src.ctypes.data, src.shape, src.dtype, dst.ctypes.data, NewWidth, NewHeight,
+                               out_dtype, (WinX, WinY, WinWidth, WinHeight), p)
+        return r, dst
+
+    def resizeImageWindowDevice(self, d_src, src_shape, in_dtype, d_dst, NewWidth, NewHeight, out_dtype, window,
+                                d_workspace, aParams=None, stream=0):
+        """Device pointers: d_src at the window's footprint (windowFootprint), d_dst receives the window;
+        src_shape is the WHOLE source's (H, W, C).  Asynchronous on `stream`.  Returns WinHeight or 0."""
+        return self._window(1, d_src, src_shape, in_dtype, d_dst, NewWidth, NewHeight, out_dtype, window,
+                            aParams or CLancIRParams(), d_workspace, stream)[0]
+
+    def windowFootprint(self, src_shape, in_dtype, NewWidth, NewHeight, out_dtype, window, aParams=None):
+        """dict of lancirb200_window_info (the source columns / rows the window reads), None where the
+        front-end returns 0."""
+        r, info, _ = self._window(2, None, src_shape, in_dtype, None, NewWidth, NewHeight, out_dtype, window,
+                                  aParams or CLancIRParams())
+        return dict(zip(("src_x0", "src_w", "src_y0", "src_h"), info)) if r > 0 else None
+
+    def windowWorkspaceBytes(self, src_shape, in_dtype, NewWidth, NewHeight, out_dtype, window, aParams=None):
+        """Device workspace bytes of resizeImageWindowDevice (0 where the front-end returns 0)."""
+        return self._window(3, None, src_shape, in_dtype, None, NewWidth, NewHeight, out_dtype, window,
+                            aParams or CLancIRParams())[2]

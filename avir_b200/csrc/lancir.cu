@@ -16,6 +16,10 @@
 // (lancir_col4_kernel / lancir_row4_kernel); other channel counts one thread per output element:
 // the column pass with threads along x (coalesced reads of every tap's row), the row pass
 // reading its taps' pixels from the fp32 intermediate through the caches.
+//
+// A destination window (lancirb200_resize_window_*) runs the same four kernels over its region: the
+// column pass over the footprint's columns and the window's rows, the row pass over the window's columns
+// (LParams x0 / y0 / fx0 / fy0 / mid_w; the whole image is the region at the origin, full size).
 
 #include <cuda_runtime.h>
 
@@ -49,8 +53,14 @@ struct LParams {
     float out_mul, clamp_max;
     int unity;
     const void* src; long long src_pitch;
-    float* mid;          // [dst_h][src_w*C]
+    float* mid;          // [win_h][mid_w*C]
     void* dst; long long dst_pitch;
+    // The destination region the passes compute (the whole image: 0, 0, dst_w, dst_h; a window: its own)
+    // and the source columns / rows the buffers start at: src holds source row fy0 onward, its column 0
+    // and the intermediate's are source column fx0, the intermediate is mid_w pixels wide (the whole
+    // image: 0, 0, src_w).  Taps clamp to the IMAGE first, then fx0 / fy0 index the buffers.
+    int x0, y0, win_w, win_h;
+    int fx0, fy0, mid_w;
 };
 
 __device__ __forceinline__ float lload(const void* p, int type, long long i) {
@@ -98,42 +108,42 @@ __device__ __forceinline__ float ltapsum(const int C, const int c, const int kl,
     return __fadd_rn(a, b);
 }
 
-// Column pass: one thread per (x, c) element of an output row; grid.y = output row.
+// Column pass: one thread per (x, c) element of an intermediate row; grid.y = output row (of the region).
 __global__ void __launch_bounds__(256) lancir_col_kernel(const __grid_constant__ LParams p) {
     const int e = blockIdx.x * blockDim.x + threadIdx.x; // element within a row
     const int y = blockIdx.y;
-    const int row_elems = p.src_w * p.C;
+    const int row_elems = p.mid_w * p.C;
     if (e >= row_elems) return;
     const int kl = p.v.kl;
-    const float* f = p.v.taps + (size_t)__ldg(p.v.phase + y) * kl;
-    const int s0 = __ldg(p.v.src_pos + y);
+    const float* f = p.v.taps + (size_t)__ldg(p.v.phase + p.y0 + y) * kl;
+    const int s0 = __ldg(p.v.src_pos + p.y0 + y);
     const void* src = p.src;
-    const int in_type = p.in_type, src_h = p.src_h;
+    const int in_type = p.in_type, src_h = p.src_h, fy0 = p.fy0;
     const long long pitch = p.src_pitch;
     const float r = ltapsum(p.C, e % p.C, kl, f, [&](int t) {
         int sy = s0 + t;
         sy = sy < 0 ? 0 : (sy >= src_h ? src_h - 1 : sy);
-        return lload(src, in_type, (long long)sy * pitch + e);
+        return lload(src, in_type, (long long)(sy - fy0) * pitch + e);
     });
     p.mid[(size_t)y * row_elems + e] = r;
 }
 
-// Row pass + output: one thread per output element; grid.y = row.
+// Row pass + output: one thread per output element of the region; grid.y = row.
 __global__ void __launch_bounds__(256) lancir_row_kernel(const __grid_constant__ LParams p) {
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
     const int y = blockIdx.y;
-    const int out_elems = p.dst_w * p.C;
+    const int out_elems = p.win_w * p.C;
     if (e >= out_elems) return;
     const int x = e / p.C, c = e - x * p.C;
     const int kl = p.h.kl;
-    const float* f = p.h.taps + (size_t)__ldg(p.h.phase + x) * kl;
-    const int s0 = __ldg(p.h.src_pos + x);
-    const float* row = p.mid + (size_t)y * p.src_w * p.C;
-    const int C = p.C, src_w = p.src_w;
+    const float* f = p.h.taps + (size_t)__ldg(p.h.phase + p.x0 + x) * kl;
+    const int s0 = __ldg(p.h.src_pos + p.x0 + x);
+    const float* row = p.mid + (size_t)y * p.mid_w * p.C;
+    const int C = p.C, src_w = p.src_w, fx0 = p.fx0;
     float v = ltapsum(C, c, kl, f, [&](int t) {
         int sx = s0 + t;
         sx = sx < 0 ? 0 : (sx >= src_w ? src_w - 1 : sx);
-        return row[(size_t)sx * C + c];
+        return row[(size_t)(sx - fx0) * C + c];
     });
     if (!p.unity) v = __fmul_rn(v, p.out_mul);
     const long long g = (long long)y * p.dst_pitch + e;
@@ -142,7 +152,8 @@ __global__ void __launch_bounds__(256) lancir_row_kernel(const __grid_constant__
         return;
     }
     int iv;
-    const bool tail = e >= (out_elems & ~3);
+    // (the tail is the last (dst_w * C) & 3 elements of a whole destination row, whatever the region)
+    const bool tail = p.x0 * C + e >= ((p.dst_w * C) & ~3);
     if (tail) {
         const float cv = v > p.clamp_max ? p.clamp_max : (v < 0.0f ? 0.0f : v);
         iv = __float2int_rz(__fadd_rn(cv, 0.5f));
@@ -192,18 +203,18 @@ constexpr int kLColRows = 32; // output rows a block of the column pass walks
 template <typename TIN, int KL>
 __global__ void __launch_bounds__(256) lancir_col4_kernel(const __grid_constant__ LParams p) {
     const int px = blockIdx.x * 256 + threadIdx.x;
-    if (px >= p.src_w) return;
+    if (px >= p.mid_w) return;
     const int y0 = blockIdx.y * kLColRows;
-    const int y1 = (y0 + kLColRows < p.dst_h) ? y0 + kLColRows : p.dst_h;
-    const int kl = KL ? KL : p.v.kl, src_h = p.src_h;
+    const int y1 = (y0 + kLColRows < p.win_h) ? y0 + kLColRows : p.win_h;
+    const int kl = KL ? KL : p.v.kl, src_h = p.src_h, fy0 = p.fy0;
     const long long pitch = p.src_pitch;
     for (int y = y0; y < y1; ++y) {
-        const float* f = p.v.taps + (size_t)__ldg(p.v.phase + y) * kl;
-        const int s0 = __ldg(p.v.src_pos + y);
+        const float* f = p.v.taps + (size_t)__ldg(p.v.phase + p.y0 + y) * kl;
+        const int s0 = __ldg(p.v.src_pos + p.y0 + y);
         auto S = [&](int t) {
             int sy = s0 + t;
             sy = sy < 0 ? 0 : (sy >= src_h ? src_h - 1 : sy);
-            return LPix<TIN>::load(p.src, (long long)sy * pitch + (long long)px * 4);
+            return LPix<TIN>::load(p.src, (long long)(sy - fy0) * pitch + (long long)px * 4);
         };
         float4 ev, od;
         if (KL) {
@@ -223,7 +234,7 @@ __global__ void __launch_bounds__(256) lancir_col4_kernel(const __grid_constant_
                 od = ladd4(od, lmul4(__ldg(f + t + 1), S(t + 1)));
             }
         }
-        reinterpret_cast<float4*>(p.mid + (size_t)y * p.src_w * 4)[px] = ladd4(ev, od);
+        reinterpret_cast<float4*>(p.mid + (size_t)y * p.mid_w * 4)[px] = ladd4(ev, od);
     }
 }
 
@@ -232,15 +243,15 @@ template <int OUT, int KL>
 __global__ void __launch_bounds__(256) lancir_row4_kernel(const __grid_constant__ LParams p) {
     const int x = blockIdx.x * 256 + threadIdx.x;
     const int y = blockIdx.y;
-    if (x >= p.dst_w) return;
-    const int kl = KL ? KL : p.h.kl, src_w = p.src_w;
-    const float* f = p.h.taps + (size_t)__ldg(p.h.phase + x) * kl;
-    const int s0 = __ldg(p.h.src_pos + x);
-    const float4* row = reinterpret_cast<const float4*>(p.mid + (size_t)y * src_w * 4);
+    if (x >= p.win_w) return;
+    const int kl = KL ? KL : p.h.kl, src_w = p.src_w, fx0 = p.fx0;
+    const float* f = p.h.taps + (size_t)__ldg(p.h.phase + p.x0 + x) * kl;
+    const int s0 = __ldg(p.h.src_pos + p.x0 + x);
+    const float4* row = reinterpret_cast<const float4*>(p.mid + (size_t)y * p.mid_w * 4);
     auto M = [&](int t) {
         int sx = s0 + t;
         sx = sx < 0 ? 0 : (sx >= src_w ? src_w - 1 : sx);
-        return row[sx];
+        return row[sx - fx0];
     };
     float4 ev, od;
     if (KL) {
@@ -279,12 +290,39 @@ __global__ void __launch_bounds__(256) lancir_row4_kernel(const __grid_constant_
             make_ushort4((unsigned short)a, (unsigned short)b, (unsigned short)c, (unsigned short)d);
 }
 
+// The source span [lo, lo + n) the outputs [i0, i0 + cnt) of an axis read: every tap position clamped to
+// the image, the min / max over the outputs' table entries (the tables need not be monotone).  Zero taps
+// count: the kernels multiply every tap, and 0 * NaN is NaN.
+void lspan(const int32_t* pos, int kl, int src_len, int i0, int cnt, int32_t* lo, int32_t* n) {
+    long long a = src_len, b = -1;
+    for (int i = i0; i < i0 + cnt; ++i) {
+        long long first = pos[i], last = (long long)pos[i] + kl - 1;
+        first = first < 0 ? 0 : (first >= src_len ? src_len - 1 : first);
+        last = last < 0 ? 0 : (last >= src_len ? src_len - 1 : last);
+        a = first < a ? first : a;
+        b = last > b ? last : b;
+    }
+    *lo = (int32_t)a;
+    *n = (int32_t)(b - a + 1);
+}
+
+// The footprint of the destination window [x0, x0 + w) x [y0, y0 + h).
+int lwindow(const int32_t* hpos, int hkl, const int32_t* vpos, int vkl, int src_w, int src_h, int dst_w, int dst_h,
+            int x0, int y0, int w, int h, lancirb200_window_info* info) {
+    if (x0 < 0 || y0 < 0 || w < 1 || h < 1 || (long long)x0 + w > dst_w || (long long)y0 + h > dst_h)
+        return fail(AVIRB200_ERR_BAD_ARG, "window empty or outside the destination");
+    lspan(hpos, hkl, src_w, x0, w, &info->src_x0, &info->src_w);
+    lspan(vpos, vkl, src_h, y0, h, &info->src_y0, &info->src_h);
+    return 0;
+}
+
 } // namespace
 
 struct lancirb200_plan {
     lancirb200_plan_desc desc;
     void* arena = nullptr;
     LAxis dv, dh;
+    std::vector<int32_t> pos_v, pos_h; // host copies of the axes' src_pos (window footprints)
     int device = 0;
     std::mutex mx;
     void* d_src = nullptr;
@@ -343,7 +381,12 @@ int lancirb200_plan_create(const lancirb200_plan_desc* d, lancirb200_plan** out)
         da.phase = reinterpret_cast<const int*>(base + off); off += avb::align_up(n, 256);
     }
     CUDA_TRY(cudaMemcpy(pl->arena, img.data(), bytes, cudaMemcpyHostToDevice));
+    pl->pos_v.assign(d->v.src_pos, d->v.src_pos + d->v.dst_len);
+    pl->pos_h.assign(d->h.src_pos, d->h.src_pos + d->h.dst_len);
+    // (the descriptor's tables are the caller's: the plan keeps no pointer to them)
     pl->desc.v.taps = nullptr; pl->desc.h.taps = nullptr;
+    pl->desc.v.src_pos = nullptr; pl->desc.h.src_pos = nullptr;
+    pl->desc.v.phase = nullptr; pl->desc.h.phase = nullptr;
     *out = pl.release();
     return 0;
 }
@@ -361,9 +404,14 @@ int lancirb200_plan_workspace_bytes(const lancirb200_plan* pl, size_t* bytes) {
     return 0;
 }
 
-int lancirb200_resize_device(const lancirb200_plan* pl, const void* d_src, size_t src_pitch,
-                             void* d_dst, size_t dst_pitch, void* d_ws, void* stream) {
-    if (!pl || !d_src || !d_dst || !d_ws) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
+} // extern "C"
+
+namespace {
+
+// Both passes over the destination region [x0, x0 + w) x [y0, y0 + h): d_src holds the source from row fy0
+// on, its column 0 is source column fx0, and the intermediate in d_ws is h rows of fw pixels.
+int lancir_region(const lancirb200_plan* pl, int x0, int y0, int w, int h, int fx0, int fw, int fy0,
+                  const void* d_src, size_t src_pitch, void* d_dst, size_t dst_pitch, void* d_ws, void* stream) {
     const lancirb200_plan_desc& d = pl->desc;
     LParams p;
     p.v = pl->dv; p.h = pl->dh;
@@ -373,8 +421,10 @@ int lancirb200_resize_device(const lancirb200_plan* pl, const void* d_src, size_
     p.src = d_src; p.src_pitch = (long long)src_pitch;
     p.mid = static_cast<float*>(d_ws);
     p.dst = d_dst; p.dst_pitch = (long long)dst_pitch;
+    p.x0 = x0; p.y0 = y0; p.win_w = w; p.win_h = h;
+    p.fx0 = fx0; p.fy0 = fy0; p.mid_w = fw;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (d.dst_h > 65535) return fail(AVIRB200_ERR_UNSUPPORTED, "image too tall");
+    if (h > 65535) return fail(AVIRB200_ERR_UNSUPPORTED, "image too tall");
     (void)cudaGetLastError(); // (a stale non-sticky error of another library is not this launch's)
     // 4-channel images whose pixels are aligned to their own size: the vector kernels
     const bool vec_in = d.channels == 4 && (src_pitch % 4) == 0 && ((uintptr_t)d_src % (4 * elem_size(d.in_type))) == 0 &&
@@ -382,7 +432,7 @@ int lancirb200_resize_device(const lancirb200_plan* pl, const void* d_src, size_
     const bool vec_out = d.channels == 4 && (dst_pitch % 4) == 0 && ((uintptr_t)d_dst % (4 * elem_size(d.out_type))) == 0 &&
                          ((uintptr_t)d_ws % 16) == 0;
     if (vec_in) {
-        dim3 g1((d.src_w + 255) / 256, (d.dst_h + kLColRows - 1) / kLColRows);
+        dim3 g1((fw + 255) / 256, (h + kLColRows - 1) / kLColRows);
 #define LCOL(KL)                                                                                        \
     do {                                                                                                \
         if (d.in_type == AVIRB200_U8) lancir_col4_kernel<unsigned char, KL><<<g1, 256, 0, st>>>(p);     \
@@ -398,11 +448,11 @@ int lancirb200_resize_device(const lancirb200_plan* pl, const void* d_src, size_
         }
 #undef LCOL
     } else {
-        dim3 g1((d.src_w * d.channels + 255) / 256, d.dst_h);
+        dim3 g1((fw * d.channels + 255) / 256, h);
         lancir_col_kernel<<<g1, 256, 0, st>>>(p);
     }
     if (vec_out) {
-        dim3 g2((d.dst_w + 255) / 256, d.dst_h);
+        dim3 g2((w + 255) / 256, h);
 #define LROW(KL)                                                                                        \
     do {                                                                                                \
         if (d.out_type == AVIRB200_U8) lancir_row4_kernel<1, KL><<<g2, 256, 0, st>>>(p);                \
@@ -418,11 +468,28 @@ int lancirb200_resize_device(const lancirb200_plan* pl, const void* d_src, size_
         }
 #undef LROW
     } else {
-        dim3 g2((d.dst_w * d.channels + 255) / 256, d.dst_h);
+        dim3 g2((w * d.channels + 255) / 256, h);
         lancir_row_kernel<<<g2, 256, 0, st>>>(p);
     }
     CUDA_TRY(cudaGetLastError());
     return 0;
+}
+
+int lancir_window(const lancirb200_plan* pl, int x0, int y0, int w, int h, lancirb200_window_info* info) {
+    const lancirb200_plan_desc& d = pl->desc;
+    return lwindow(pl->pos_h.data(), pl->dh.kl, pl->pos_v.data(), pl->dv.kl, d.src_w, d.src_h, d.dst_w, d.dst_h, x0, y0,
+                   w, h, info);
+}
+
+} // namespace
+
+extern "C" {
+
+int lancirb200_resize_device(const lancirb200_plan* pl, const void* d_src, size_t src_pitch,
+                             void* d_dst, size_t dst_pitch, void* d_ws, void* stream) {
+    if (!pl || !d_src || !d_dst || !d_ws) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
+    const lancirb200_plan_desc& d = pl->desc;
+    return lancir_region(pl, 0, 0, d.dst_w, d.dst_h, 0, d.src_w, 0, d_src, src_pitch, d_dst, dst_pitch, d_ws, stream);
 }
 
 int lancirb200_resize_host(lancirb200_plan* pl, const void* h_src, size_t src_pitch, void* h_dst,
@@ -455,6 +522,95 @@ int lancirb200_resize_host(lancirb200_plan* pl, const void* h_src, size_t src_pi
     if (r != 0) return r;
     CUDA_TRY(cudaMemcpy2DAsync(h_dst, dst_pitch * elem_size(d.out_type), pl->d_dst, out_row, out_row,
                                 d.dst_h, cudaMemcpyDeviceToHost, pl->stream));
+    CUDA_TRY(cudaStreamSynchronize(pl->stream));
+    return 0;
+}
+
+int lancirb200_window_query(const lancirb200_plan* pl, int x0, int y0, int w, int h, lancirb200_window_info* info) {
+    if (!pl || !info) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
+    return lancir_window(pl, x0, y0, w, h, info);
+}
+
+int lancirb200_window_query_desc(const lancirb200_plan_desc* d, int x0, int y0, int w, int h,
+                                 lancirb200_window_info* info) {
+    if (!d || !info) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
+    if (d->src_w < 1 || d->src_h < 1 || d->dst_w < 1 || d->dst_h < 1 || !d->h.src_pos || !d->v.src_pos ||
+        d->h.dst_len < d->dst_w || d->v.dst_len < d->dst_h || d->h.kernel_len < 1 || d->v.kernel_len < 1)
+        return fail(AVIRB200_ERR_BAD_ARG, "bad geometry or axis tables");
+    return lwindow(d->h.src_pos, d->h.kernel_len, d->v.src_pos, d->v.kernel_len, d->src_w, d->src_h, d->dst_w,
+                   d->dst_h, x0, y0, w, h, info);
+}
+
+int lancirb200_window_workspace_bytes(const lancirb200_plan* pl, int x0, int y0, int w, int h, size_t* bytes) {
+    if (!pl || !bytes) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
+    lancirb200_window_info wi;
+    const int r = lancir_window(pl, x0, y0, w, h, &wi);
+    if (r != 0) return r;
+    *bytes = (size_t)h * wi.src_w * pl->desc.channels * sizeof(float);
+    return 0;
+}
+
+int lancirb200_resize_window_device(const lancirb200_plan* pl, int x0, int y0, int w, int h, const void* d_src,
+                                    size_t src_pitch, void* d_dst, size_t dst_pitch, void* d_ws, void* stream) {
+    if (!pl || !d_src || !d_dst || !d_ws) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
+    lancirb200_window_info wi;
+    const int r = lancir_window(pl, x0, y0, w, h, &wi);
+    if (r != 0) return r;
+    const int C = pl->desc.channels;
+    if (src_pitch < (size_t)wi.src_w * C || dst_pitch < (size_t)w * C)
+        return fail(AVIRB200_ERR_BAD_ARG, "pitch smaller than a row");
+    return lancir_region(pl, x0, y0, w, h, wi.src_x0, wi.src_w, wi.src_y0, d_src, src_pitch, d_dst, dst_pitch, d_ws,
+                         stream);
+}
+
+int lancirb200_resize_window_host(lancirb200_plan* pl, int x0, int y0, int w, int h, const void* h_src,
+                                  size_t src_pitch, void* h_dst, size_t dst_pitch) {
+    if (!pl || !h_src || !h_dst) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
+    const lancirb200_plan_desc& d = pl->desc;
+    lancirb200_window_info wi;
+    int r = lancir_window(pl, x0, y0, w, h, &wi);
+    if (r != 0) return r;
+    if (src_pitch < (size_t)d.src_w * d.channels || dst_pitch < (size_t)w * d.channels)
+        return fail(AVIRB200_ERR_BAD_ARG, "pitch smaller than a row");
+    std::lock_guard<std::mutex> lk(pl->mx);
+    // the call runs on the plan's device; the caller's current device is restored on every exit
+    struct DeviceGuard {
+        int prev = -1;
+        ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
+    } guard;
+    {
+        int cur = -1;
+        CUDA_TRY(cudaGetDevice(&cur));
+        if (cur != pl->device) {
+            CUDA_TRY(cudaSetDevice(pl->device));
+            guard.prev = cur;
+        }
+    }
+    const size_t in_el = elem_size(d.in_type), out_el = elem_size(d.out_type);
+    const size_t in_row = (size_t)wi.src_w * d.channels * in_el, out_row = (size_t)w * d.channels * out_el;
+    const size_t ws = (size_t)h * wi.src_w * d.channels * sizeof(float);
+    if (!pl->stream) CUDA_TRY(cudaStreamCreateWithFlags(&pl->stream, cudaStreamNonBlocking));
+    if (pl->src_bytes < in_row * wi.src_h) {
+        cudaFree(pl->d_src); pl->d_src = nullptr; pl->src_bytes = 0;
+        CUDA_TRY(cudaMalloc(&pl->d_src, in_row * wi.src_h)); pl->src_bytes = in_row * wi.src_h;
+    }
+    if (pl->dst_bytes < out_row * h) {
+        cudaFree(pl->d_dst); pl->d_dst = nullptr; pl->dst_bytes = 0;
+        CUDA_TRY(cudaMalloc(&pl->d_dst, out_row * h)); pl->dst_bytes = out_row * h;
+    }
+    if (pl->ws_bytes < ws) {
+        cudaFree(pl->d_ws); pl->d_ws = nullptr; pl->ws_bytes = 0;
+        CUDA_TRY(cudaMalloc(&pl->d_ws, ws)); pl->ws_bytes = ws;
+    }
+    // the footprint only
+    const char* fsrc = static_cast<const char*>(h_src) + ((size_t)wi.src_y0 * src_pitch + (size_t)wi.src_x0 * d.channels) * in_el;
+    CUDA_TRY(cudaMemcpy2DAsync(pl->d_src, in_row, fsrc, src_pitch * in_el, in_row, wi.src_h, cudaMemcpyHostToDevice,
+                               pl->stream));
+    r = lancir_region(pl, x0, y0, w, h, wi.src_x0, wi.src_w, wi.src_y0, pl->d_src, (size_t)wi.src_w * d.channels,
+                      pl->d_dst, (size_t)w * d.channels, pl->d_ws, pl->stream);
+    if (r != 0) return r;
+    CUDA_TRY(cudaMemcpy2DAsync(h_dst, dst_pitch * out_el, pl->d_dst, out_row, out_row, h, cudaMemcpyDeviceToHost,
+                               pl->stream));
     CUDA_TRY(cudaStreamSynchronize(pl->stream));
     return 0;
 }

@@ -326,6 +326,37 @@ int lancirb200_resize_device(const lancirb200_plan* plan, const void* d_src, siz
 int lancirb200_resize_host(lancirb200_plan* plan, const void* h_src, size_t src_pitch,
                            void* h_dst, size_t dst_pitch);
 
+/* Destination windows of a LANCIR plan, as avirb200_*window* for AVIR: the window
+ * [x0, x0 + w) x [y0, y0 + h) of the plan's full resize, bit-identical to the same pixels of
+ * lancirb200_resize_device.  The column pass runs over the footprint's columns and the window's rows
+ * only, the row pass over the window's columns only.  Windows must be non-empty and lie inside the
+ * destination (AVIRB200_ERR_BAD_ARG, before any CUDA call); a window may be at most 65535 rows tall,
+ * whatever the plan's height. */
+typedef struct lancirb200_window_info {
+    int32_t src_x0, src_w;   /* source columns the window reads, clamped to the image (reads past an */
+    int32_t src_y0, src_h;   /*   edge replicate the edge), and source rows */
+} lancirb200_window_info;
+
+/* The footprint: every tap position of every window output, clamped to the image, min / max per axis
+ * (zero-valued taps included).  Pure host arithmetic on the plan's own copy of the tables. */
+int lancirb200_window_query(const lancirb200_plan* plan, int x0, int y0, int w, int h, lancirb200_window_info* info);
+/* Same, from a descriptor alone (no device needed). */
+int lancirb200_window_query_desc(const lancirb200_plan_desc* desc, int x0, int y0, int w, int h,
+                                 lancirb200_window_info* info);
+/* Workspace of one window call: the intermediate, h x src_w(footprint) pixels of floats. */
+int lancirb200_window_workspace_bytes(const lancirb200_plan* plan, int x0, int y0, int w, int h, size_t* bytes);
+/* d_src points at the footprint's first pixel (source pixel (src_x0, src_y0)) and holds its
+ * src_w x src_h pixels; d_dst points at the window's first pixel and receives w x h pixels.  Pitches in
+ * elements; asynchronous on `stream`, no allocation. */
+int lancirb200_resize_window_device(const lancirb200_plan* plan, int x0, int y0, int w, int h, const void* d_src,
+                                    size_t src_pitch, void* d_dst, size_t dst_pitch, void* d_workspace,
+                                    void* stream);
+/* The same with HOST buffers: h_src is the WHOLE source image (only the footprint is copied to the
+ * device), h_dst receives the w x h window.  Pageable or page-locked memory; synchronises; the
+ * caller's current device is unchanged afterwards. */
+int lancirb200_resize_window_host(lancirb200_plan* plan, int x0, int y0, int w, int h, const void* h_src,
+                                  size_t src_pitch, void* h_dst, size_t dst_pitch);
+
 /* ---- misc ----------------------------------------------------------------------------- */
 
 const char* avirb200_status_string(int status);

@@ -224,6 +224,94 @@ public:
                            &Params);
     }
 
+    // GPU extension: the destination window [WinX, WinX + WinWidth) x [WinY, WinY + WinHeight) of
+    // resizeImage(SrcBuf, SrcWidth, SrcHeight, NewBuf, NewWidth, NewHeight, ElCount, aParams), bit for
+    // bit, reading only the window's source footprint (windowFootprint).  SrcBuf is the WHOLE source
+    // (Params.SrcSSize its scanline size), NewBuf receives the window (Params.NewSSize its scanline
+    // size, < 1: WinWidth * ElCount).  Returns WinHeight, or 0 as resizeImage does and for a window
+    // that is empty or not inside the destination.  Every window of one geometry shares the plan
+    // resizeImage caches.
+    template <typename Tin, typename Tout>
+    int resizeImageWindow(const Tin* const SrcBuf, const int SrcWidth, const int SrcHeight,
+                          Tout* const NewBuf, const int NewWidth, const int NewHeight, const int ElCount,
+                          const int WinX, const int WinY, const int WinWidth, const int WinHeight,
+                          const CLancIRParams* const aParams = nullptr) {
+        if ((SrcBuf == nullptr) | ((const void*)SrcBuf == (const void*)NewBuf) ||
+            !windowArgs(SrcWidth, SrcHeight, NewBuf, NewWidth, NewHeight, WinX, WinY, WinWidth, WinHeight, aParams))
+            return 0;
+        const CLancIRParams& Params = params(aParams);
+        const size_t NewScanlineSize =
+            (size_t)(Params.NewSSize < 1 ? WinWidth * ElCount : Params.NewSSize);
+        if ((SrcWidth == 0) | (SrcHeight == 0)) { // lancir.h:414-426, for the window's pixels
+            Tout* op = NewBuf;
+            for (int i = 0; i < WinHeight; i++) {
+                std::memset(op, 0, (size_t)WinWidth * ElCount * sizeof(Tout));
+                op += NewScanlineSize;
+            }
+            return WinHeight;
+        }
+        const size_t SrcScanlineSize =
+            (size_t)(Params.SrcSSize < 1 ? SrcWidth * ElCount : Params.SrcSSize);
+        if (!ensurePlan<Tin, Tout>(SrcWidth, SrcHeight, NewWidth, NewHeight, ElCount, Params))
+            return 0;
+        if (lancirb200_resize_window_host(Plan, WinX, WinY, WinWidth, WinHeight, SrcBuf, SrcScanlineSize, NewBuf,
+                                          NewScanlineSize) != 0)
+            return 0;
+        return WinHeight;
+    }
+
+    // The same with DEVICE pointers, asynchronous on `Stream` (a cudaStream_t): dSrcBuf points at the
+    // footprint's first pixel and holds its src_w x src_h pixels (Params.SrcSSize elements apart, < 1:
+    // src_w * ElCount), dNewBuf receives the window, `Workspace` holds windowWorkspaceBytes() bytes of
+    // device memory.  Returns WinHeight or 0; an empty source has no footprint and returns 0.
+    template <typename Tin, typename Tout>
+    int resizeImageWindowDevice(const Tin* const dSrcBuf, const int SrcWidth, const int SrcHeight,
+                                Tout* const dNewBuf, const int NewWidth, const int NewHeight, const int ElCount,
+                                const int WinX, const int WinY, const int WinWidth, const int WinHeight,
+                                void* const Workspace, void* const Stream = nullptr,
+                                const CLancIRParams* const aParams = nullptr) {
+        lancirb200_window_info wi;
+        if ((dSrcBuf == nullptr) | ((const void*)dSrcBuf == (const void*)dNewBuf) | (Workspace == nullptr) ||
+            windowFootprint<Tin, Tout>(SrcWidth, SrcHeight, NewWidth, NewHeight, ElCount, WinX, WinY, WinWidth,
+                                       WinHeight, &wi, aParams) == 0)
+            return 0;
+        const CLancIRParams& Params = params(aParams);
+        const size_t SrcScanlineSize = (size_t)(Params.SrcSSize < 1 ? wi.src_w * ElCount : Params.SrcSSize);
+        const size_t NewScanlineSize = (size_t)(Params.NewSSize < 1 ? WinWidth * ElCount : Params.NewSSize);
+        if (lancirb200_resize_window_device(Plan, WinX, WinY, WinWidth, WinHeight, dSrcBuf, SrcScanlineSize, dNewBuf,
+                                            NewScanlineSize, Workspace, Stream) != 0)
+            return 0;
+        return WinHeight;
+    }
+
+    // The source pixels a window reads (clamped to the image) into *Info.  Returns WinHeight or 0.
+    template <typename Tin, typename Tout>
+    int windowFootprint(const int SrcWidth, const int SrcHeight, const int NewWidth, const int NewHeight,
+                        const int ElCount, const int WinX, const int WinY, const int WinWidth, const int WinHeight,
+                        lancirb200_window_info* const Info, const CLancIRParams* const aParams = nullptr) {
+        if ((Info == nullptr) | (SrcWidth < 1) | (SrcHeight < 1) ||
+            !windowArgs(SrcWidth, SrcHeight, Info, NewWidth, NewHeight, WinX, WinY, WinWidth, WinHeight, aParams) ||
+            !ensurePlan<Tin, Tout>(SrcWidth, SrcHeight, NewWidth, NewHeight, ElCount, params(aParams)) ||
+            lancirb200_window_query(Plan, WinX, WinY, WinWidth, WinHeight, Info) != 0)
+            return 0;
+        return WinHeight;
+    }
+
+    // Bytes of device workspace resizeImageWindowDevice needs for the window, or 0 where it would
+    // return 0.
+    template <typename Tin, typename Tout>
+    size_t windowWorkspaceBytes(const int SrcWidth, const int SrcHeight, const int NewWidth, const int NewHeight,
+                                const int ElCount, const int WinX, const int WinY, const int WinWidth,
+                                const int WinHeight, const CLancIRParams* const aParams = nullptr) {
+        lancirb200_window_info wi;
+        size_t b = 0;
+        if (windowFootprint<Tin, Tout>(SrcWidth, SrcHeight, NewWidth, NewHeight, ElCount, WinX, WinY, WinWidth,
+                                       WinHeight, &wi, aParams) == 0 ||
+            lancirb200_window_workspace_bytes(Plan, WinX, WinY, WinWidth, WinHeight, &b) != 0)
+            return 0;
+        return b;
+    }
+
     // Host-only: fills the C descriptor for a call (tables owned by *this).
     template <typename Tin, typename Tout>
     bool buildDescriptor(lancirb200_plan_desc& d, const int SrcWidth, const int SrcHeight,
@@ -277,6 +365,24 @@ private:
                    la == o.la;
         }
     } Cur{-1, -1, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+
+    static const CLancIRParams& params(const CLancIRParams* const aParams) {
+        static const CLancIRParams DefParams;
+        return aParams != nullptr ? *aParams : DefParams;
+    }
+
+    // resizeImage's argument rules (lancir.h:392-408) for the window calls, plus a non-empty window
+    // inside the destination.
+    static bool windowArgs(const int SrcWidth, const int SrcHeight, const void* const NewBuf, const int NewWidth,
+                           const int NewHeight, const int WinX, const int WinY, const int WinWidth,
+                           const int WinHeight, const CLancIRParams* const aParams) {
+        if ((SrcWidth < 0) | (SrcHeight < 0) | (NewWidth <= 0) | (NewHeight <= 0) | (NewBuf == nullptr))
+            return false;
+        if ((WinX < 0) | (WinY < 0) | (WinWidth <= 0) | (WinHeight <= 0) | (WinX > NewWidth - WinWidth) |
+            (WinY > NewHeight - WinHeight))
+            return false;
+        return params(aParams).la >= 2.0;
+    }
 
     static void fill(lancirb200_axis_desc& a, const lancir_detail::FilterSet& f,
                      const lancir_detail::AxisTables& t, int src_len, int dst_len) {

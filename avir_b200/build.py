@@ -143,8 +143,10 @@ def _build_host(force=False):
 
 
 def build_oracles():
-    """C port always; the upstream-compiled oracle only where /root/reference exists."""
+    """C port always; the upstream-compiled oracle only where /root/reference exists (oracle/Makefile, and
+    oracle/types.mk for CLancIR's double and uint32_t buffers)."""
     _run(["make", "-C", os.path.join(ROOT, "oracle"), "all"])
+    _run(["make", "-C", os.path.join(ROOT, "oracle"), "-f", "types.mk", "all"])
 
 
 def build_emul(force=False):

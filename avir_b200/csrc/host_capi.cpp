@@ -9,6 +9,7 @@
 #include <cstring>
 #include <memory>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "avir_b200.h"
@@ -122,6 +123,10 @@ void run1(const CallArgs& a, OpArgs& o) {
 }
 
 int run0(const CallArgs& a, OpArgs& o) {
+    if (a.tin < AVIRB200_U8 || a.tin > AVIRB200_F64 || a.tout < AVIRB200_U8 || a.tout > AVIRB200_F64) {
+        g_err = "CImageResizer: element type code outside 0..3 (uint8_t, uint16_t, float, double)";
+        return -1;
+    }
     try {
         switch (a.mirror) {
         case 1: run1<avir::fpclass_float4>(a, o); break;
@@ -304,6 +309,34 @@ avir::CLancIR& lancir_obj() {
     return obj;
 }
 
+template <class Tin, class F>
+bool lancir_out(int tout, const void* src, void* dst, F& f) {
+    switch (tout) {
+    case AVIRB200_U8: f((const Tin*)src, (uint8_t*)dst); return true;
+    case AVIRB200_U16: f((const Tin*)src, (uint16_t*)dst); return true;
+    case AVIRB200_F32: f((const Tin*)src, (float*)dst); return true;
+    case AVIRB200_F64: f((const Tin*)src, (double*)dst); return true;
+    case AVIRB200_U32: f((const Tin*)src, (uint32_t*)dst); return true;
+    }
+    return false;
+}
+
+// Calls f((const Tin*)src, (Tout*)dst) with the element types of the codes tin / tout (avirb200_dtype, the
+// five CLancIR types); false, without a call, for a code outside 0..4.
+template <class F>
+bool lancir_types(int tin, int tout, const void* src, void* dst, F f) {
+    switch (tin) {
+    case AVIRB200_U8: return lancir_out<uint8_t>(tout, src, dst, f);
+    case AVIRB200_U16: return lancir_out<uint16_t>(tout, src, dst, f);
+    case AVIRB200_F32: return lancir_out<float>(tout, src, dst, f);
+    case AVIRB200_F64: return lancir_out<double>(tout, src, dst, f);
+    case AVIRB200_U32: return lancir_out<uint32_t>(tout, src, dst, f);
+    }
+    return false;
+}
+
+template <class P> using elem_t = std::remove_const_t<std::remove_pointer_t<P> >;
+
 } // namespace
 
 extern "C" {
@@ -315,24 +348,13 @@ int lancirb200_host_resize(int tin, int tout, const void* src, int sw, int sh, v
     avir::CLancIR& obj = lancir_obj();
     avir::CLancIRParams p(srcssize, newssize, kx, ky, ox, oy);
     p.la = la;
-    if (tin < 0 || tin > 2 || tout < 0 || tout > 2) { // u8 / u16 / float buffers only (no double)
-        g_err = "lancirb200_host_resize: element type code outside 0..2";
+    int r = 0;
+    if (!lancir_types(tin, tout, src, dst,
+                      [&](const auto* s, auto* d) { r = obj.resizeImage(s, sw, sh, d, nw, nh, ch, &p); })) {
+        g_err = "lancirb200_host_resize: element type code outside 0..4";
         return -1;
     }
-#define LR(TI, TO) return obj.resizeImage((const TI*)src, sw, sh, (TO*)dst, nw, nh, ch, &p)
-    switch (tin * 3 + tout) {
-    case 0: LR(uint8_t, uint8_t);
-    case 1: LR(uint8_t, uint16_t);
-    case 2: LR(uint8_t, float);
-    case 3: LR(uint16_t, uint8_t);
-    case 4: LR(uint16_t, uint16_t);
-    case 5: LR(uint16_t, float);
-    case 6: LR(float, uint8_t);
-    case 7: LR(float, uint16_t);
-    case 8: LR(float, float);
-    }
-#undef LR
-    return 0;
+    return r;
 }
 
 struct LancirDescHandle {
@@ -340,27 +362,18 @@ struct LancirDescHandle {
     lancirb200_plan_desc desc;
 };
 
-// Host-only LANCIR descriptor (u8 or float I/O selects the output-stage constants).
+// Host-only LANCIR descriptor (the element types select the output-stage constants); null for a type
+// code outside 0..4.
 void* lancirb200_host_desc_create(int tin, int tout, int sw, int sh, int nw, int nh, int ch,
                                   double kx, double ky, double ox, double oy, double la) {
-    if (tin < 0 || tin > 2 || tout < 0 || tout > 2) return nullptr;
     LancirDescHandle* h = new LancirDescHandle();
     avir::CLancIRParams p(0, 0, kx, ky, ox, oy);
     p.la = la;
     bool ok = false;
-#define LD(TI, TO) ok = h->obj.buildDescriptor<TI, TO>(h->desc, sw, sh, nw, nh, ch, p); break
-    switch (tin * 3 + tout) {
-    case 0: LD(uint8_t, uint8_t);
-    case 1: LD(uint8_t, uint16_t);
-    case 2: LD(uint8_t, float);
-    case 3: LD(uint16_t, uint8_t);
-    case 4: LD(uint16_t, uint16_t);
-    case 5: LD(uint16_t, float);
-    case 6: LD(float, uint8_t);
-    case 7: LD(float, uint16_t);
-    case 8: LD(float, float);
-    }
-#undef LD
+    if (!lancir_types(tin, tout, nullptr, nullptr, [&](const auto* s, auto* d) {
+            ok = h->obj.buildDescriptor<elem_t<decltype(s)>, elem_t<decltype(d)> >(h->desc, sw, sh, nw, nh, ch, p);
+        }))
+        g_err = "lancirb200_host_desc_create: element type code outside 0..4";
     if (!ok) { delete h; return nullptr; }
     return h;
 }
@@ -374,8 +387,8 @@ int lancirb200_host_window(int op, int tin, int tout, const void* src, int sw, i
                            int ch, int srcssize, int newssize, double kx, double ky, double ox, double oy,
                            double la, int wx, int wy, int ww, int wh, void* d_workspace, void* stream, int* info,
                            long long* bytes) {
-    if (op < 0 || op > 3 || tin < 0 || tin > 2 || tout < 0 || tout > 2) {
-        g_err = "lancirb200_host_window: op outside 0..3 or element type code outside 0..2";
+    if (op < 0 || op > 3 || tin < AVIRB200_U8 || tin > AVIRB200_U32 || tout < AVIRB200_U8 || tout > AVIRB200_U32) {
+        g_err = "lancirb200_host_window: op outside 0..3 or element type code outside 0..4";
         return -1;
     }
     avir::CLancIR& obj = lancir_obj();
@@ -384,26 +397,14 @@ int lancirb200_host_window(int op, int tin, int tout, const void* src, int sw, i
     lancirb200_window_info wi{};
     size_t nb = 0;
     int r = 0;
-#define LW(TI, TO)                                                                                              \
-    if (op == 0) r = obj.resizeImageWindow((const TI*)src, sw, sh, (TO*)dst, nw, nh, ch, wx, wy, ww, wh, &p);   \
-    else if (op == 1)                                                                                           \
-        r = obj.resizeImageWindowDevice((const TI*)src, sw, sh, (TO*)dst, nw, nh, ch, wx, wy, ww, wh,           \
-                                        d_workspace, stream, &p);                                               \
-    else if (op == 2) r = obj.windowFootprint<TI, TO>(sw, sh, nw, nh, ch, wx, wy, ww, wh, &wi, &p);             \
-    else r = (nb = obj.windowWorkspaceBytes<TI, TO>(sw, sh, nw, nh, ch, wx, wy, ww, wh, &p)) != 0;              \
-    break
-    switch (tin * 3 + tout) {
-    case 0: LW(uint8_t, uint8_t);
-    case 1: LW(uint8_t, uint16_t);
-    case 2: LW(uint8_t, float);
-    case 3: LW(uint16_t, uint8_t);
-    case 4: LW(uint16_t, uint16_t);
-    case 5: LW(uint16_t, float);
-    case 6: LW(float, uint8_t);
-    case 7: LW(float, uint16_t);
-    case 8: LW(float, float);
-    }
-#undef LW
+    lancir_types(tin, tout, src, dst, [&](const auto* s, auto* d) {
+        using TI = elem_t<decltype(s)>;
+        using TO = elem_t<decltype(d)>;
+        if (op == 0) r = obj.resizeImageWindow(s, sw, sh, d, nw, nh, ch, wx, wy, ww, wh, &p);
+        else if (op == 1) r = obj.resizeImageWindowDevice(s, sw, sh, d, nw, nh, ch, wx, wy, ww, wh, d_workspace, stream, &p);
+        else if (op == 2) r = obj.windowFootprint<TI, TO>(sw, sh, nw, nh, ch, wx, wy, ww, wh, &wi, &p);
+        else r = (nb = obj.windowWorkspaceBytes<TI, TO>(sw, sh, nw, nh, ch, wx, wy, ww, wh, &p)) != 0;
+    });
     if (info != nullptr) std::memcpy(info, &wi, sizeof wi);
     if (bytes != nullptr) *bytes = (long long)nb;
     return r;

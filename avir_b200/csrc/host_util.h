@@ -15,7 +15,14 @@ namespace avb {
 int fail(int code, const std::string& msg);
 
 // Bytes of one element of an avirb200_dtype.
-inline size_t elem_size(int t) { return t == AVIRB200_U8 ? 1 : (t == AVIRB200_U16 ? 2 : (t == AVIRB200_F64 ? 8 : 4)); }
+inline size_t elem_size(int t) {
+    switch (t) {
+    case AVIRB200_U8: return 1;
+    case AVIRB200_U16: return 2;
+    case AVIRB200_F64: return 8;
+    case AVIRB200_F32: case AVIRB200_U32: default: return 4;
+    }
+}
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 

@@ -20,9 +20,16 @@
 // A destination window (lancirb200_resize_window_*) runs the same four kernels over its region: the
 // column pass over the footprint's columns and the window's rows, the row pass over the window's columns
 // (LParams x0 / y0 / fx0 / fy0 / mid_w; the whole image is the region at the origin, full size).
+//
+// Element types (upstream lancir.h:373-381): u8, u16, float, double and uint32_t, read and written by the
+// kernels themselves (lload / LPix on input, the row passes' stores on output).  Input is (float) v,
+// nearest-even (__double2float_rn / __uint2float_rn; float subnormals are kept, the build does not flush
+// them).  double output is (double) of the float result; uint32_t output is u16's output stored 32 bits
+// wide, except that a NaN in the half-up tail stores x86's (int)NaN = INT_MIN, as upstream's roundclamp.
 
 #include <cuda_runtime.h>
 
+#include <climits>
 #include <cstdint>
 #include <cstring>
 #include <memory>
@@ -66,6 +73,8 @@ struct LParams {
 __device__ __forceinline__ float lload(const void* p, int type, long long i) {
     if (type == AVIRB200_U8) return (float)((const unsigned char*)p)[i];
     if (type == AVIRB200_U16) return (float)((const unsigned short*)p)[i];
+    if (type == AVIRB200_F64) return __double2float_rn(((const double*)p)[i]);
+    if (type == AVIRB200_U32) return __uint2float_rn(((const unsigned int*)p)[i]);
     return ((const float*)p)[i];
 }
 
@@ -151,18 +160,24 @@ __global__ void __launch_bounds__(256) lancir_row_kernel(const __grid_constant__
         ((float*)p.dst)[g] = v;
         return;
     }
+    if (p.out_type == AVIRB200_F64) {
+        ((double*)p.dst)[g] = (double)v;
+        return;
+    }
     int iv;
     // (the tail is the last (dst_w * C) & 3 elements of a whole destination row, whatever the region)
     const bool tail = p.x0 * C + e >= ((p.dst_w * C) & ~3);
     if (tail) {
+        // NaN passes the clamp; x86's (int)NaN is INT_MIN: 0 once truncated to u8 / u16, 2147483648 as u32
         const float cv = v > p.clamp_max ? p.clamp_max : (v < 0.0f ? 0.0f : v);
-        iv = __float2int_rz(__fadd_rn(cv, 0.5f));
+        iv = cv != cv ? INT_MIN : __float2int_rz(__fadd_rn(cv, 0.5f));
     } else {
         const float cv = fmaxf(fminf(v, p.clamp_max), 0.0f);
         iv = __float2int_rn(cv);
     }
     if (p.out_type == AVIRB200_U8) ((unsigned char*)p.dst)[g] = (unsigned char)iv;
-    else ((unsigned short*)p.dst)[g] = (unsigned short)iv;
+    else if (p.out_type == AVIRB200_U16) ((unsigned short*)p.dst)[g] = (unsigned short)iv;
+    else ((unsigned int*)p.dst)[g] = (unsigned int)iv;
 }
 
 // ---- 4-channel images: one thread per PIXEL, vector loads and stores ----------------------------
@@ -186,6 +201,20 @@ template <> struct LPix<unsigned short> {
 template <> struct LPix<float> {
     static __device__ __forceinline__ float4 load(const void* p, long long i) {
         return *reinterpret_cast<const float4*>(static_cast<const float*>(p) + i);
+    }
+};
+template <> struct LPix<double> { // a 32-byte pixel: two 16-byte loads
+    static __device__ __forceinline__ float4 load(const void* p, long long i) {
+        const double2* q = reinterpret_cast<const double2*>(static_cast<const double*>(p) + i);
+        const double2 a = q[0], b = q[1];
+        return make_float4(__double2float_rn(a.x), __double2float_rn(a.y), __double2float_rn(b.x),
+                           __double2float_rn(b.y));
+    }
+};
+template <> struct LPix<unsigned int> {
+    static __device__ __forceinline__ float4 load(const void* p, long long i) {
+        const uint4 v = *reinterpret_cast<const uint4*>(static_cast<const unsigned int*>(p) + i);
+        return make_float4(__uint2float_rn(v.x), __uint2float_rn(v.y), __uint2float_rn(v.z), __uint2float_rn(v.w));
     }
 };
 
@@ -238,7 +267,7 @@ __global__ void __launch_bounds__(256) lancir_col4_kernel(const __grid_constant_
     }
 }
 
-// OUT: 0 float, 1 u8, 2 u16
+// OUT: 0 float, 1 u8, 2 u16, 3 double, 4 uint32_t
 template <int OUT, int KL>
 __global__ void __launch_bounds__(256) lancir_row4_kernel(const __grid_constant__ LParams p) {
     const int x = blockIdx.x * 256 + threadIdx.x;
@@ -278,6 +307,12 @@ __global__ void __launch_bounds__(256) lancir_row4_kernel(const __grid_constant_
         *reinterpret_cast<float4*>(static_cast<float*>(p.dst) + g) = v;
         return;
     }
+    if (OUT == 3) { // two 16-byte stores
+        double2* q = reinterpret_cast<double2*>(static_cast<double*>(p.dst) + g);
+        q[0] = make_double2((double)v.x, (double)v.y);
+        q[1] = make_double2((double)v.z, (double)v.w);
+        return;
+    }
     // (a row of 4-channel pixels has no (NewWidth*C) & 3 tail: every element rounds nearest-even)
     const float cm = p.clamp_max;
     const int a = __float2int_rn(fmaxf(fminf(v.x, cm), 0.0f)), b = __float2int_rn(fmaxf(fminf(v.y, cm), 0.0f));
@@ -285,9 +320,12 @@ __global__ void __launch_bounds__(256) lancir_row4_kernel(const __grid_constant_
     if (OUT == 1)
         *reinterpret_cast<uchar4*>(static_cast<unsigned char*>(p.dst) + g) =
             make_uchar4((unsigned char)a, (unsigned char)b, (unsigned char)c, (unsigned char)d);
-    else
+    else if (OUT == 2)
         *reinterpret_cast<ushort4*>(static_cast<unsigned short*>(p.dst) + g) =
             make_ushort4((unsigned short)a, (unsigned short)b, (unsigned short)c, (unsigned short)d);
+    else
+        *reinterpret_cast<uint4*>(static_cast<unsigned int*>(p.dst) + g) =
+            make_uint4((unsigned int)a, (unsigned int)b, (unsigned int)c, (unsigned int)d);
 }
 
 // The source span [lo, lo + n) the outputs [i0, i0 + cnt) of an axis read: every tap position clamped to
@@ -338,6 +376,9 @@ int lancirb200_plan_create(const lancirb200_plan_desc* d, lancirb200_plan** out)
     if (d == nullptr || out == nullptr) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
     *out = nullptr;
     if (d->channels < 1 || d->channels > 4) return fail(AVIRB200_ERR_BAD_ARG, "channels must be 1..4");
+    for (const int t : {d->in_type, d->out_type})
+        if (t < AVIRB200_U8 || t > AVIRB200_U32)
+            return fail(AVIRB200_ERR_BAD_ARG, "element type must be U8, U16, F32, F64 or U32 (0..4)");
     if (d->v.kernel_len < 4 || d->h.kernel_len < 4 || ((d->v.kernel_len | d->h.kernel_len) & 1))
         return fail(AVIRB200_ERR_BAD_ARG, "kernel length must be even and >= 4");
     if (d->src_w < 1 || d->src_h < 1 || d->dst_w < 1 || d->dst_h < 1)
@@ -437,6 +478,8 @@ int lancir_region(const lancirb200_plan* pl, int x0, int y0, int w, int h, int f
     do {                                                                                                \
         if (d.in_type == AVIRB200_U8) lancir_col4_kernel<unsigned char, KL><<<g1, 256, 0, st>>>(p);     \
         else if (d.in_type == AVIRB200_U16) lancir_col4_kernel<unsigned short, KL><<<g1, 256, 0, st>>>(p); \
+        else if (d.in_type == AVIRB200_F64) lancir_col4_kernel<double, KL><<<g1, 256, 0, st>>>(p);      \
+        else if (d.in_type == AVIRB200_U32) lancir_col4_kernel<unsigned int, KL><<<g1, 256, 0, st>>>(p); \
         else lancir_col4_kernel<float, KL><<<g1, 256, 0, st>>>(p);                                      \
     } while (0)
         switch (pl->dv.kl) { // la = 3: 6 taps when upsizing, 12 at k = 2, 18 at k = 3, 24 at k = 4
@@ -457,6 +500,8 @@ int lancir_region(const lancirb200_plan* pl, int x0, int y0, int w, int h, int f
     do {                                                                                                \
         if (d.out_type == AVIRB200_U8) lancir_row4_kernel<1, KL><<<g2, 256, 0, st>>>(p);                \
         else if (d.out_type == AVIRB200_U16) lancir_row4_kernel<2, KL><<<g2, 256, 0, st>>>(p);          \
+        else if (d.out_type == AVIRB200_F64) lancir_row4_kernel<3, KL><<<g2, 256, 0, st>>>(p);          \
+        else if (d.out_type == AVIRB200_U32) lancir_row4_kernel<4, KL><<<g2, 256, 0, st>>>(p);          \
         else lancir_row4_kernel<0, KL><<<g2, 256, 0, st>>>(p);                                          \
     } while (0)
         switch (pl->dh.kl) {

@@ -40,8 +40,16 @@ typedef enum avirb200_status {
  * F64: upstream narrows double input with a (float) cast in packScanline and widens the float
  * result with a (double) cast in unpackScanline (avir.h:2803-2806, 3168-3171); the library
  * does the same casts on the device (resize_device / resize_host; the sharded calls and the
- * per-pass entry points take U8 / U16 / F32 only). */
-typedef enum avirb200_dtype { AVIRB200_U8 = 0, AVIRB200_U16 = 1, AVIRB200_F32 = 2, AVIRB200_F64 = 3 } avirb200_dtype;
+ * per-pass entry points take U8 / U16 / F32 only).
+ * U32: LANCIR plans only (upstream lancir.h treats uint32_t as uint16_t): read as (float) v, no clamp on
+ * input, output clamped to [0, 65535] and stored 32 bits wide.  AVIR plans take U8 / U16 / F32 / F64. */
+typedef enum avirb200_dtype {
+    AVIRB200_U8 = 0,
+    AVIRB200_U16 = 1,
+    AVIRB200_F32 = 2,
+    AVIRB200_F64 = 3,
+    AVIRB200_U32 = 4
+} avirb200_dtype;
 
 /* Step kinds of a 1-D filtering chain (upstream CImageResizerFilterStep, avir.h:2568-2728). */
 typedef enum avirb200_step_kind {
@@ -309,7 +317,7 @@ typedef struct lancirb200_axis_desc {
 
 typedef struct lancirb200_plan_desc {
     int32_t src_w, src_h, dst_w, dst_h, channels;
-    int32_t in_type, out_type;
+    int32_t in_type, out_type; /* avirb200_dtype: U8, U16, F32, F64 or U32 */
     float out_mul;          /* lancir.h:526-533 */
     int32_t is_unity_mul;
     float clamp_max;        /* 255 / 65535 for integer output */
@@ -318,6 +326,13 @@ typedef struct lancirb200_plan_desc {
 
 typedef struct lancirb200_plan lancirb200_plan;
 
+/* Element types, as upstream's CLancIR (lancir.h:373-381): the kernels read and write every type
+ * natively.  Input: (float) v, rounded to nearest-even (F64 values beyond float's range become +-Inf,
+ * float subnormals stay subnormal; U32 is exact up to 2^24 and not clamped).  F64 output: (double) of
+ * the float result (times out_mul unless is_unity_mul), no clamp.  U32 output: as U16 -- clamped to
+ * [0, clamp_max], nearest-even, the last (dst_w * channels) & 3 elements of a row (int)(v + 0.5f) --
+ * stored 32 bits wide; a NaN in that tail stores x86's (int)NaN, 2147483648, as upstream does.  A type
+ * code outside 0..4 is AVIRB200_ERR_BAD_ARG, before any CUDA call. */
 int lancirb200_plan_create(const lancirb200_plan_desc* desc, lancirb200_plan** out);
 void lancirb200_plan_destroy(lancirb200_plan* plan);
 int lancirb200_plan_workspace_bytes(const lancirb200_plan* plan, size_t* bytes);

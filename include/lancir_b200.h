@@ -6,6 +6,8 @@
 // 1/1000 phase quantisation); the two filtering passes (columns first, then rows) and the
 // output conversion run as sm_90a kernels behind the C ABI in avirb200.h.
 //
+// Element types: uint8_t, uint16_t, float, double and uint32_t, for Tin and Tout alike (lancir.h:373-381).
+//
 // Bit-exact scope: upstream's AVX build.  Its tap-sum tree differs per channel count
 // (resize1..resize4, lancir.h:2101-2515); the kernels mirror each of the four.
 // There is no CPU fallback.
@@ -167,10 +169,19 @@ inline void positions(AxisTables& at, FilterSet& fs, int dst_len, double o, doub
     }
 }
 
-template <typename T> struct dtype_of;
+// Buffer element types (upstream lancir.h:373-381): uint8_t, uint16_t, float, double, and uint32_t, which
+// upstream treats as uint16_t.  Upstream leaves signed and larger integer types unsupported (they compile
+// there and give garbage); here they do not compile.
+template <typename T> struct dtype_of {
+    static_assert(sizeof(T) == 0,
+                  "CLancIR element types are uint8_t, uint16_t, float, double and uint32_t (lancir.h:373-381)");
+    static constexpr int value = -1;
+};
 template <> struct dtype_of<uint8_t> { static constexpr int value = AVIRB200_U8; };
 template <> struct dtype_of<uint16_t> { static constexpr int value = AVIRB200_U16; };
 template <> struct dtype_of<float> { static constexpr int value = AVIRB200_F32; };
+template <> struct dtype_of<double> { static constexpr int value = AVIRB200_F64; };
+template <> struct dtype_of<uint32_t> { static constexpr int value = AVIRB200_U32; };
 
 } // namespace lancir_detail
 

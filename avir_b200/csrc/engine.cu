@@ -106,7 +106,9 @@ struct avirb200_plan {
     // pipelined resize_host: copy-in / copy-out streams and per-band events
     cudaStream_t stream_in = nullptr, stream_out = nullptr;
     std::vector<cudaEvent_t> ev_in, ev_out, ev_d2h, ev_slot; // (+ staged copies of pageable buffers)
-    mutable int last_launches = 0;
+    // launches of the last call that counted them; calls on one plan from several threads each store their
+    // own count (relaxed: the value is some one call's, never a mix)
+    mutable std::atomic<int> last_launches{0};
     // options (avirb200_plan_set_option)
     // 1..3-channel images on the 4-channel kernels (streaming / tile): the source is widened to
     // 4-channel pixels in a scratch copy, both passes run as for RGBA (channels never mix; the
@@ -223,12 +225,10 @@ int launch_generic(const PassParams& p, const PassConfig& c, cudaStream_t st) {
     if (grid.x == 0 || grid.y == 0) return 0;
     if (grid.y > 65535) return fail(AVIRB200_ERR_UNSUPPORTED, "image too large for generic grid");
     if (p.sum_mode == AVIRB200_SUM_DIL8) {
-        CUDA_TRY(cudaFuncSetAttribute(generic_pass_kernel<AVIRB200_SUM_DIL8>,
-                                      cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c.smem));
+        CUDA_TRY(raise_smem_limit(reinterpret_cast<const void*>(generic_pass_kernel<AVIRB200_SUM_DIL8>), c.smem));
         generic_pass_kernel<AVIRB200_SUM_DIL8><<<grid, 256, c.smem, st>>>(p);
     } else {
-        CUDA_TRY(cudaFuncSetAttribute(generic_pass_kernel<AVIRB200_SUM_INL>,
-                                      cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c.smem));
+        CUDA_TRY(raise_smem_limit(reinterpret_cast<const void*>(generic_pass_kernel<AVIRB200_SUM_INL>), c.smem));
         generic_pass_kernel<AVIRB200_SUM_INL><<<grid, 256, c.smem, st>>>(p);
     }
     CUDA_TRY(cudaGetLastError());
@@ -253,12 +253,15 @@ struct PassRoute {
     PassFamily family;
     PassRequest k;      // the request as the kernels see it: a widened plan's scratch copies
     FastFootprint fpnt; // kFamilyTile: the footprint of the request's range
+    const int* tiles = nullptr; // kFamilyTile: the range's tile table
 };
 
 // The kernel family that runs the pass `req`: the first that applies of the streaming kernel, the tile
 // kernel and the generic kernel.  The 4-channel kernels (streaming, tile) move whole pixels: the row pass's
 // source pixels and the column pass's channel pairs must be aligned to their size, the intermediate to 16
-// bytes.  The tile kernel also needs the footprint of the request's tiles to fit its shared memory.
+// bytes.  The tile kernel also needs the table of the request's range, built ahead by plan creation, a window or
+// shard query or the banded host call (a launch never builds one: no allocation, no synchronous copy), and the
+// footprint of the range's tiles to fit its shared memory.
 PassRoute pass_family(const avirb200_plan* pl, const PassRequest& req) {
     PassRoute r;
     r.k = req;
@@ -278,10 +281,11 @@ PassRoute pass_family(const avirb200_plan* pl, const PassRequest& req) {
                                       ((uintptr_t)k.dst % 16) == 0;
     const avs::StreamAxisPlan& sa = k.is_v ? pl->stream_v : pl->stream_h;
     const bool tile_ok = k.is_v ? pl->fast.v_ok : pl->fast.h_ok;
+    const FastPass& fp = k.is_v ? pl->fast.v : pl->fast.h;
     if (pl->opt_family == 0 && sa.chain != 0 && aligned) {
         r.family = kFamilyStream;
-    } else if (pl->opt_family != 1 && tile_ok && aligned &&
-               (r.fpnt = fast_range_footprint(k.is_v ? pl->fast.v : pl->fast.h, k.out0, k.out1)).smem <= kFastSmemBudget) {
+    } else if (pl->opt_family != 1 && tile_ok && aligned && (r.tiles = fast_tile_table_find(fp, k.out0, k.out1)) != nullptr &&
+               (r.fpnt = fast_range_footprint(fp, k.out0, k.out1)).smem <= kFastSmemBudget) {
         r.family = kFamilyTile;
     } else {
         r.family = kFamilyGeneric;
@@ -353,8 +357,8 @@ int run_pass(const avirb200_plan* pl, const PassRequest& req, cudaStream_t st, i
                                pl->sm_count, st) != 0)
             e = fail(AVIRB200_ERR_CUDA, std::string("streaming ") + pass + " launch failed");
     } else if (r.family == kFamilyTile) {
-        if (fast_pass(k.is_v ? pl->fast.v : pl->fast.h, k, r.fpnt, pixel_stage(d, pl->d_lut), d.sum_mode, pl->sm_count,
-                      st) != 0)
+        if (fast_pass(k.is_v ? pl->fast.v : pl->fast.h, k, r.fpnt, r.tiles, pixel_stage(d, pl->d_lut), d.sum_mode,
+                      pl->sm_count, st) != 0)
             e = fail(AVIRB200_ERR_CUDA, std::string("fast ") + pass + " launch failed");
     } else {
         e = generic_pass(pl, k, p4 ? 4 : d.channels, st);
@@ -1294,16 +1298,19 @@ int avirb200_plan_workspace_bytes(const avirb200_plan* pl, size_t* bytes) {
     return 0;
 }
 
-int avirb200_plan_last_launches(const avirb200_plan* pl) { return pl ? pl->last_launches : 0; }
+int avirb200_plan_last_launches(const avirb200_plan* pl) {
+    return pl ? pl->last_launches.load(std::memory_order_relaxed) : 0;
+}
 
 } // extern "C"
 
 namespace {
 
 // The whole image (win null), or the destination window [x0, x0 + w) x [y0, y0 + h) with its footprint
-// *win: d_src holds the footprint, d_dst receives the window.
+// *win: d_src holds the footprint, d_dst receives the window.  *n_launches (when given): the call's launches.
 int resize_region(const avirb200_plan* pl, const avirb200_window_info* win, int x0, int y0, int w, int h,
-                  const void* d_src, size_t src_pitch, void* d_dst, size_t dst_pitch, void* d_ws, void* stream) {
+                  const void* d_src, size_t src_pitch, void* d_dst, size_t dst_pitch, void* d_ws, void* stream,
+                  int* n_launches = nullptr) {
     const avirb200_plan_desc& d = pl->desc;
     const int src_w = win ? win->src_w : d.src_w, src_h = win ? win->src_h : d.src_h;
     if (src_pitch < (size_t)src_w * d.channels || dst_pitch < (size_t)w * d.channels)
@@ -1382,7 +1389,8 @@ int resize_region(const avirb200_plan* pl, const avirb200_window_info* win, int 
         ++launches;
         CUDA_TRY(cudaGetLastError());
     }
-    pl->last_launches = launches;
+    pl->last_launches.store(launches, std::memory_order_relaxed);
+    if (n_launches != nullptr) *n_launches = launches;
     return r;
 }
 
@@ -1507,11 +1515,14 @@ int avirb200_resize_device_batch(const avirb200_plan* pl, int n, const void* con
     int total = 0;
     for (int i = 0; i < n; ++i) {
         // frames share the workspace: the stream keeps frame i's column pass ahead of frame i+1's row pass
-        const int r = avirb200_resize_device(pl, d_srcs[i], src_pitch, d_dsts[i], dst_pitch, d_ws, stream);
+        if (d_srcs[i] == nullptr || d_dsts[i] == nullptr) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
+        int launches = 0;
+        const int r = resize_region(pl, nullptr, 0, 0, pl->desc.dst_w, pl->desc.dst_h, d_srcs[i], src_pitch, d_dsts[i],
+                                    dst_pitch, d_ws, stream, &launches);
         if (r != 0) return r;
-        total += pl->last_launches;
+        total += launches;
     }
-    pl->last_launches = total;
+    pl->last_launches.store(total, std::memory_order_relaxed);
     return 0;
 }
 
@@ -1573,6 +1584,8 @@ int avirb200_resize_host(avirb200_plan* pl, const void* h_src, size_t src_pitch,
         nb /= 2;
     }
     if (nb >= 2) {
+        // the tile kernel's tables of the bands' destination rows (a launch does not build them)
+        for (int b = 0; b < nb; ++b) fast_prepare_range(pl->fast, si[b].dst_row0, si[b].dst_row0 + si[b].dst_rows);
         if (pl->stream_in == nullptr) CUDA_TRY(cudaStreamCreateWithFlags(&pl->stream_in, cudaStreamNonBlocking));
         if (pl->stream_out == nullptr) CUDA_TRY(cudaStreamCreateWithFlags(&pl->stream_out, cudaStreamNonBlocking));
         while ((int)pl->ev_in.size() < nb) {
@@ -1682,7 +1695,7 @@ int avirb200_resize_host(avirb200_plan* pl, const void* h_src, size_t src_pitch,
         }
         int r = col_band(nb - 1);
         if (r != 0) return r;
-        pl->last_launches = launches;
+        pl->last_launches.store(launches, std::memory_order_relaxed);
         CUDA_TRY(cudaStreamSynchronize(pl->stream_out));
         CUDA_TRY(cudaStreamSynchronize(pl->stream));
         if (drainer.t.joinable()) drainer.t.join(); // the last bands reach the caller's memory
@@ -1771,7 +1784,7 @@ int avirb200_resize_sharded(const avirb200_plan* cpl, void* comm, int rank, int 
     if (nranks <= 1) {
         r = run_pass(pl, row, st, &launches);
         if (r == 0) r = run_pass(pl, col, st, &launches);
-        pl->last_launches = launches;
+        pl->last_launches.store(launches, std::memory_order_relaxed);
         return r;
     }
     if (comm == nullptr) return fail(AVIRB200_ERR_BAD_ARG, "sharded resize needs a communicator");
@@ -1875,7 +1888,7 @@ int avirb200_resize_sharded(const avirb200_plan* cpl, void* comm, int rank, int 
         }
         // the pushes read this call's workspace: the caller's stream does not end before them
         if (pushed) CUDA_TRY(cudaStreamWaitEvent(st, pl->ev_x1, 0));
-        pl->last_launches = launches;
+        pl->last_launches.store(launches, std::memory_order_relaxed);
         return r;
     }
     // NCCL schedule: whole row pass, send/recv group, column pass, one stream
@@ -1893,7 +1906,7 @@ int avirb200_resize_sharded(const avirb200_plan* cpl, void* comm, int rank, int 
     }
     NCCL_TRY(nc->GroupEnd());
     r = run_pass(pl, col, st, &launches);
-    pl->last_launches = launches;
+    pl->last_launches.store(launches, std::memory_order_relaxed);
     return r;
 }
 
@@ -1995,7 +2008,7 @@ int avirb200_resize_sharded_local(const avirb200_plan* pl, int nranks, const voi
         for (int r = 0; r < nranks && e == 0; ++r) e = run_pass(pl, row[r], st, &launches);
         for (int r = 0; r < nranks && e == 0; ++r) e = run_pass(pl, col[r], st, &launches);
         cudaFreeAsync(boxes, st);
-        pl->last_launches = launches;
+        pl->last_launches.store(launches, std::memory_order_relaxed);
         return e;
     }
     for (int r = 0; r < nranks; ++r) { // every band's row pass
@@ -2017,7 +2030,7 @@ int avirb200_resize_sharded_local(const avirb200_plan* pl, int nranks, const voi
         int e = run_pass(pl, col[r], st, &launches);
         if (e != 0) return e;
     }
-    pl->last_launches = launches;
+    pl->last_launches.store(launches, std::memory_order_relaxed);
     return 0;
 }
 

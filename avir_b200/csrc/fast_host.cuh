@@ -19,7 +19,8 @@ struct FastPass {
     std::vector<std::vector<float> > eff_taps;
     std::vector<std::vector<int> > eff_idx, src_pos;
     void* arena = nullptr;
-    // per-launch-geometry tables of tile ranges (device), built on first use
+    // per-range device tables of tile ranges: built by fast_tile_table_build (plan creation, the
+    // window / shard queries, the banded host call), only looked up on the launch path
     mutable std::map<std::pair<int, int>, int*> range_tabs;
     mutable std::mutex tabs_mx;
 };
@@ -30,6 +31,24 @@ struct FastPlan {
 };
 
 const size_t kFastSmemBudget = (227 * 1024) / kFastBlocksPerSM - 2048; // per block
+
+// Lets `kernel` launch with at least `bytes` of dynamic shared memory on the current device, never lowering
+// what it allowed before.  The limit belongs to the function, not to a launch: a plain cudaFuncSetAttribute
+// with each launch's own size, from threads sharing a plan (or plans of one device), could lower it under
+// another thread's larger launch of the same kernel, and that launch would fail.
+inline cudaError_t raise_smem_limit(const void* kernel, size_t bytes) {
+    static std::mutex mx;
+    static std::map<std::pair<int, const void*>, size_t> limits; // (device, kernel) -> bytes allowed
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    std::lock_guard<std::mutex> lk(mx);
+    size_t& cur = limits[std::make_pair(dev, kernel)];
+    if (bytes <= cur) return cudaSuccess;
+    e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e == cudaSuccess) cur = bytes;
+    return e;
+}
 
 // A resize step all of whose outputs use effective phase 0 (the only one): integer ratios.
 inline bool hax_uniform(const FastAxis& hax, int i) {
@@ -220,16 +239,16 @@ inline int fast_upload(FastPass& fp) {
     return 0;
 }
 
-inline const int* fast_tile_table(const FastPass& fp, int out0, int out1);
+inline const int* fast_tile_table_build(const FastPass& fp, int out0, int out1);
 
-// Builds the tile table of a destination-row range ahead of its first launch (sharded calls,
-// banded host calls): called from the host-side queries every such caller makes first.
+// Builds the tile table of a destination-row range ahead of its launches (sharded calls, banded host
+// calls, windows): called from the host-side queries every such caller makes first.
 inline void fast_prepare_range(const FastPlan& f, int out0, int out1) {
-    if (f.v_ok && out1 > out0) fast_tile_table(f.v, out0, out1);
+    if (f.v_ok && out1 > out0) fast_tile_table_build(f.v, out0, out1);
 }
 // The same for the row pass's intermediate columns [out0, out1) (windows).
 inline void fast_prepare_columns(const FastPlan& f, int out0, int out1) {
-    if (f.h_ok && out1 > out0) fast_tile_table(f.h, out0, out1);
+    if (f.h_ok && out1 > out0) fast_tile_table_build(f.h, out0, out1);
 }
 
 inline void fast_plan_init(FastPlan& f, const DevAxis& h_host, const DevAxis& v_host,
@@ -255,7 +274,7 @@ inline void fast_plan_init(FastPlan& f, const DevAxis& h_host, const DevAxis& v_
         if (fp.fpnt.smem > kFastSmemBudget) continue;
         // the whole-image tile table is built and uploaded here, not at the first launch (launches
         // stay asynchronous and allocation-free; shard ranges: fast_prepare_range())
-        fp.ok = (fast_tile_table(fp, 0, hs[a]->dst_len) != nullptr);
+        fp.ok = (fast_tile_table_build(fp, 0, hs[a]->dst_len) != nullptr);
     }
     f.h_ok = f.h.ok;
     f.v_ok = f.v.ok;
@@ -282,8 +301,7 @@ inline int fast_launch(const FastParams& p, size_t smem, int sum_mode, int sm_co
     cudaError_t e = cudaSuccess;
 #define AVB_LAUNCH_K(...)                                                                          \
     do {                                                                                           \
-        e = cudaFuncSetAttribute(fast_pass_kernel<__VA_ARGS__>,                                    \
-                                 cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);          \
+        e = raise_smem_limit(reinterpret_cast<const void*>(fast_pass_kernel<__VA_ARGS__>), smem);  \
         if (e == cudaSuccess) fast_pass_kernel<__VA_ARGS__><<<grid, kFastThreads, smem, st>>>(p);  \
     } while (0)
     // chain-specialised instantiations (the BASELINE configs); anything else runs the
@@ -326,8 +344,9 @@ inline int fast_launch(const FastParams& p, size_t smem, int sum_mode, int sm_co
 }
 
 // Device table of the index ranges every tile of [out0, out1) needs: per tile
-// (kFastMaxSteps + 1) x (a, b): entry 0 = source tile, entry i + 1 = outputs of step i.
-inline const int* fast_tile_table(const FastPass& fp, int out0, int out1) {
+// (kFastMaxSteps + 1) x (a, b): entry 0 = source tile, entry i + 1 = outputs of step i.  Built once per
+// range; allocates and copies synchronously, so never called from a launch.
+inline const int* fast_tile_table_build(const FastPass& fp, int out0, int out1) {
     std::lock_guard<std::mutex> lk(fp.tabs_mx);
     const std::pair<int, int> key(out0, out1);
     auto it = fp.range_tabs.find(key);
@@ -366,6 +385,14 @@ inline const int* fast_tile_table(const FastPass& fp, int out0, int out1) {
     return d;
 }
 
+// The table fast_tile_table_build made for [out0, out1), or null: the launch path's only access (a range
+// without a table runs on the generic kernel, with the same bits).
+inline const int* fast_tile_table_find(const FastPass& fp, int out0, int out1) {
+    std::lock_guard<std::mutex> lk(fp.tabs_mx);
+    const auto it = fp.range_tabs.find(std::pair<int, int>(out0, out1));
+    return it == fp.range_tabs.end() ? nullptr : it->second;
+}
+
 // Picks the (single) resize step whose one effective phase goes into the kernel parameters.
 inline void fast_set_const_taps(FastParams& p, const FastPass& fp) {
     p.debug = 0; // (the kernels' perf-experiment branches are never enabled from the library)
@@ -397,10 +424,11 @@ inline FastFootprint fast_range_footprint(const FastPass& fp, int out0, int out1
     return fast_footprint_all(fp.hax, fp.tile_out, out0, out1, fp.raw);
 }
 
-// Launches the pass q (its buffers as the kernel sees them) with the footprint fast_range_footprint gave.
+// Launches the pass q (its buffers as the kernel sees them) with the footprint fast_range_footprint gave and
+// the range's table fast_tile_table_find gave.
 // Returns 0 = launched, -1 = launch error, -2 = more tiles than a launch can count.
-inline int fast_pass(const FastPass& fp, const PassRequest& q, const FastFootprint& fpnt, const PixelStage& px,
-                     int sum_mode, int sm_count, cudaStream_t st) {
+inline int fast_pass(const FastPass& fp, const PassRequest& q, const FastFootprint& fpnt, const int* tile_ranges,
+                     const PixelStage& px, int sum_mode, int sm_count, cudaStream_t st) {
     FastParams p;
     memset(&p, 0, sizeof p);
     p.ax = fp.ax;
@@ -410,8 +438,7 @@ inline int fast_pass(const FastPass& fp, const PassRequest& q, const FastFootpri
     p.out0 = q.out0; p.out1 = q.out1;
     fast_set_footprint(p, fpnt);
     fast_set_const_taps(p, fp);
-    p.tile_ranges = fast_tile_table(fp, q.out0, q.out1);
-    if (p.tile_ranges == nullptr) return -1;
+    p.tile_ranges = tile_ranges;
     p.src = q.src; p.src_pitch = (long long)q.src_pitch; p.src_type = q.src_type;
     p.src_row_base = q.src_base;
     p.dst = q.dst; p.dst_pitch = (long long)q.dst_pitch; p.dst_type = q.dst_type;

@@ -542,7 +542,19 @@ int lancirb200_resize_host(lancirb200_plan* pl, const void* h_src, size_t src_pi
     if (!pl || !h_src || !h_dst) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
     const lancirb200_plan_desc& d = pl->desc;
     std::lock_guard<std::mutex> lk(pl->mx);
-    CUDA_TRY(cudaSetDevice(pl->device));
+    // the call runs on the plan's device; the caller's current device is restored on every exit
+    struct DeviceGuard {
+        int prev = -1;
+        ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
+    } guard;
+    {
+        int cur = -1;
+        CUDA_TRY(cudaGetDevice(&cur));
+        if (cur != pl->device) {
+            CUDA_TRY(cudaSetDevice(pl->device));
+            guard.prev = cur;
+        }
+    }
     const size_t in_row = (size_t)d.src_w * d.channels * elem_size(d.in_type);
     const size_t out_row = (size_t)d.dst_w * d.channels * elem_size(d.out_type);
     size_t ws = 0;

@@ -169,7 +169,8 @@ int avirb200_col_pass_device(const avirb200_plan* plan, const void* d_workspace,
 int avirb200_resize_host(avirb200_plan* plan, const void* h_src, size_t src_pitch, void* h_dst,
                          size_t dst_pitch);
 
-/* Number of kernel launches the last avirb200_resize_device on this plan issued. */
+/* Number of kernel launches the last avirb200_resize_device on this plan issued.  Under concurrent
+ * calls on one plan it is the count of one of those calls. */
 int avirb200_plan_last_launches(const avirb200_plan* plan);
 
 /* Video / batch entry: `n` frames of the plan's geometry, one launch pair per frame, all on
@@ -196,8 +197,13 @@ typedef struct avirb200_window_info {
     int32_t mid_row0, mid_rows; /* intermediate rows the column pass reads (= the source rows) */
 } avirb200_window_info;
 
-/* The footprint of a window.  Also builds the per-range device tables the window's passes use,
- * so that avirb200_resize_window_device stays asynchronous and allocation-free. */
+/* The footprint of a window.  Also builds the tile kernel's device tables of the window's column and
+ * row ranges (once per window: an allocation and a synchronous copy; avirb200_window_workspace_bytes
+ * does the same).  A window queried first runs its passes on the tile kernel where the plan has it; a
+ * window never queried runs them on the generic kernel, with the same bits (a 1920 x 1080 window of
+ * 7680 x 4320 -> 5120 x 2880 RGBA u8 took 4.2 x as long on an H100 80GB HBM3 at 700 W:
+ * profiles/h100_streams.txt).  avirb200_resize_window_device never builds a table: it stays
+ * asynchronous, allocation-free and capturable into a CUDA graph either way. */
 int avirb200_window_query(const avirb200_plan* plan, int x0, int y0, int w, int h, avirb200_window_info* info);
 /* Same, from a descriptor alone (pure host arithmetic, no device needed). */
 int avirb200_window_query_desc(const avirb200_plan_desc* desc, int x0, int y0, int w, int h,
@@ -338,6 +344,8 @@ void lancirb200_plan_destroy(lancirb200_plan* plan);
 int lancirb200_plan_workspace_bytes(const lancirb200_plan* plan, size_t* bytes);
 int lancirb200_resize_device(const lancirb200_plan* plan, const void* d_src, size_t src_pitch,
                              void* d_dst, size_t dst_pitch, void* d_workspace, void* stream);
+/* Host buffers in and out, on the plan's device; synchronises; the caller's current device is unchanged
+ * afterwards. */
 int lancirb200_resize_host(lancirb200_plan* plan, const void* h_src, size_t src_pitch,
                            void* h_dst, size_t dst_pitch);
 

@@ -499,6 +499,9 @@ int window_compute(const avirb200_plan* pl, int x0, int y0, int w, int h, avirb2
 // Quirk kept: the de-interleaved class stores a row as consecutive channel planes and runs them
 // one after the other, so the "Dith[j-1] +=" of pixel 0 of plane c+1 lands on the last pixel of
 // plane c (avir_dil.h:964, rsdj[-1] with j = 0):  D_{y+1}[c][W-1] gains + 0.207305*Noise_{c+1}(0).
+// A band of a sharded call runs the same kernel over its own rows: its first group takes the D row of
+// the band above (carry_in) instead of zeros, and its last row publishes its D row (carry_out) to the
+// band below the way lane 31 publishes to the next group.  The result does not depend on the banding.
 struct ErrdParams {
     const float* src;     // [H][W*C] gamma-corrected floats (the column pass's output)
     void* dst;
@@ -508,7 +511,23 @@ struct ErrdParams {
     float tr_mul, tr_mul_inv, pk_out;
     float* boundary;      // [groups][W*C]
     int* progress;        // [groups]: pixels of the group's last row whose D values are published
+    // carry_in: D of row 0 (null: zeros, the image's first row).  carry_in_prog null: carry_in is complete
+    // before the launch; else a progress word (seq << 32 | pixels published), see errd_carry_ready.
+    const float* carry_in;
+    const unsigned long long* carry_in_prog;
+    // carry_out: D of the row below row H-1 (null: no band below).  carry_out_prog null: nobody waits for
+    // it (a copy follows the kernel); else seq << 32 | pixels published, after a system-scope fence.
+    float* carry_out;
+    unsigned long long* carry_out_prog;
+    unsigned seq; // the call's sequence number: a progress word names its call, so it is never reset
 };
+
+// Whether progress word v (seq << 32 | pixels) shows pixel pix of call seq published.  The sequence halves are
+// compared modulo 2^32 (as the halo flags are): a word of an earlier call is older even after seq wraps.
+__device__ __forceinline__ bool errd_carry_ready(unsigned long long v, unsigned seq, int pix) {
+    const unsigned hi = (unsigned)(v >> 32), lo = (unsigned)v;
+    return hi == seq ? lo > (unsigned)pix : (int)(hi - seq) > 0;
+}
 
 template <int C>
 __global__ void __launch_bounds__(32) errd_kernel(const __grid_constant__ ErrdParams p) {
@@ -521,7 +540,9 @@ __global__ void __launch_bounds__(32) errd_kernel(const __grid_constant__ ErrdPa
     volatile int* prog_in = p.progress + (g > 0 ? g - 1 : 0);
     volatile int* prog_out = p.progress + g;
     const bool publish = (lane == 31) && ((g + 1) * 32 < p.H);
+    const bool carry = p.carry_out != nullptr && y == p.H - 1; // the band's last row: publishes to the band below
     int seen = 0; // lane 0: pixels the group above is known to have published
+    unsigned long long cseen = 0; // group 0, lane 0: the band above's progress word as last read
     float nm1[C], c3p[C], part[C], dn[C], v[C], vn[C], n2first[C];
 #pragma unroll
     for (int c = 0; c < C; ++c) { nm1[c] = c3p[c] = part[c] = dn[c] = n2first[c] = 0.0f; v[c] = vn[c] = 0.0f; }
@@ -539,9 +560,21 @@ __global__ void __launch_bounds__(32) errd_kernel(const __grid_constant__ ErrdPa
         for (int c = 0; c < C; ++c) din[c] = __shfl_up_sync(0xffffffffu, dn[c], 1);
         // ... or, for the group's first row, from the group above (row 0 of the image: zero)
         if (lane == 0 && on) {
-            if (g == 0) {
+            if (g == 0 && p.carry_in == nullptr) {
 #pragma unroll
                 for (int c = 0; c < C; ++c) din[c] = 0.0f;
+            } else if (g == 0) {
+                if (p.carry_in_prog != nullptr && !errd_carry_ready(cseen, p.seq, pix)) {
+                    long long spins = 0;
+                    while (!errd_carry_ready(cseen = *reinterpret_cast<const volatile unsigned long long*>(p.carry_in_prog),
+                                             p.seq, pix)) {
+                        if (++spins > (1ll << 31)) __trap(); // the band above never delivered: fail instead of hanging
+                        __nanosleep(64);
+                    }
+                    __threadfence_system();
+                }
+#pragma unroll
+                for (int c = 0; c < C; ++c) din[c] = __ldcv(p.carry_in + (size_t)pix * C + c);
             } else {
                 while (seen <= pix) seen = *prog_in;
                 __threadfence();
@@ -596,6 +629,19 @@ __global__ void __launch_bounds__(32) errd_kernel(const __grid_constant__ ErrdPa
                 for (int c = 0; c < C; ++c) __stcg(bnd_out + (size_t)q * C + c, dn[c]);
                 __threadfence();
                 *prog_out = q + 1;
+            }
+        }
+        if (carry) {
+            const int q = (on && pix >= 1) ? pix - 1 : ((pix == W) ? W - 1 : -1);
+            if (q >= 0) {
+#pragma unroll
+                for (int c = 0; c < C; ++c) p.carry_out[(size_t)q * C + c] = dn[c];
+                // (every 32 pixels and the last: one system-scope fence per 32 peer stores)
+                if (p.carry_out_prog != nullptr && ((q & 31) == 31 || q == W - 1)) {
+                    __threadfence_system();
+                    asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(p.carry_out_prog),
+                                 "l"(((unsigned long long)p.seq << 32) | (unsigned)(q + 1)) : "memory");
+                }
             }
         }
     }
@@ -671,28 +717,29 @@ __global__ void __launch_bounds__(256) widen_f32_kernel(const float* __restrict_
 }
 
 // error diffusion: per 32-row group one row of boundary values + one progress counter
-int errd_groups(const avirb200_plan* pl) { return (pl->desc.dst_h + 31) / 32; }
+int errd_groups(int rows) { return (rows + 31) / 32; }
 
 // The workspace of one call: byte offsets of its segments, in this order, each 256-byte aligned.
 // A call covers src_rows x src_cols source pixels, mid_rows x dst_cols intermediate pixels and
 // dst_rows x dst_cols destination pixels (the whole image, a shard's band or a window and its footprint).
 //   mid        the intermediate: mid_rows rows of mid_pitch(dst_cols) floats (at offset 0)
-//   in32       float copy of a double source                                  } whole-image and window
-//   out32      float copy of the destination (double output, error diffusion) } calls only: sharded
-//   errd_bnd   error diffusion: boundary rows, one per 32-row group           } and per-pass calls refuse
-//   errd_prog  error diffusion: progress counters                             } such plans (windows: errd)
+//   in32       float copy of a double source
+//   out32      float copy of the destination (double output, error diffusion)
+//   errd_bnd   error diffusion: boundary rows, one per 32-row group of the call's destination rows
+//   errd_prog  error diffusion: progress counters
+//   errd_carry error diffusion, shards only: the D rows received from the band above and sent to the band
+//              below when they travel through NCCL (the mailbox schedules carry them in the mailbox)
 //   src4       the widened source      } widened plans (pad4) only
 //   dst4       the widened destination }
-// Segments a plan does not use are empty.
+// Segments a plan does not use are empty (windows refuse error diffusion).
 struct WsLayout {
-    size_t in32, out32, errd_bnd, errd_prog, src4, dst4, total;
+    size_t in32, out32, errd_bnd, errd_prog, errd_carry, src4, dst4, total;
 };
-WsLayout ws_layout(const avirb200_plan* pl, int mid_rows, int src_rows, int dst_rows, bool whole, int src_cols,
+WsLayout ws_layout(const avirb200_plan* pl, int mid_rows, int src_rows, int dst_rows, bool shard, int src_cols,
                    int dst_cols) {
     const avirb200_plan_desc& d = pl->desc;
-    const bool f64_in = whole && pl->io_in_type == AVIRB200_F64;
-    const bool f32_out = whole && (pl->io_out_type == AVIRB200_F64 || pl->errd);
-    const bool errd = whole && pl->errd;
+    const bool f64_in = pl->io_in_type == AVIRB200_F64;
+    const bool f32_out = pl->io_out_type == AVIRB200_F64 || pl->errd;
     WsLayout w;
     size_t off = align_up((size_t)mid_rows * mid_pitch(pl, dst_cols) * sizeof(float), 256);
     auto seg = [&](bool on, size_t bytes) {
@@ -702,8 +749,9 @@ WsLayout ws_layout(const avirb200_plan* pl, int mid_rows, int src_rows, int dst_
     };
     w.in32 = seg(f64_in, (size_t)src_cols * src_rows * d.channels * sizeof(float));
     w.out32 = seg(f32_out, (size_t)dst_cols * dst_rows * d.channels * sizeof(float));
-    w.errd_bnd = seg(errd, (size_t)errd_groups(pl) * d.dst_w * d.channels * sizeof(float));
-    w.errd_prog = seg(errd, (size_t)errd_groups(pl) * sizeof(int));
+    w.errd_bnd = seg(pl->errd, (size_t)errd_groups(dst_rows) * d.dst_w * d.channels * sizeof(float));
+    w.errd_prog = seg(pl->errd, (size_t)errd_groups(dst_rows) * sizeof(int));
+    w.errd_carry = seg(pl->errd && shard, 2 * (size_t)d.dst_w * d.channels * sizeof(float));
     w.src4 = seg(pl->pad4, (size_t)src_rows * src_cols * 4 * elem_size(d.in_type));
     w.dst4 = seg(pl->pad4, (size_t)dst_rows * dst_cols * 4 * elem_size(d.out_type));
     w.total = off;
@@ -712,15 +760,80 @@ WsLayout ws_layout(const avirb200_plan* pl, int mid_rows, int src_rows, int dst_
 // The whole image's layout (resize_device, the per-pass entry points, the banded host call).
 WsLayout ws_layout(const avirb200_plan* pl) {
     const avirb200_plan_desc& d = pl->desc;
-    return ws_layout(pl, d.src_h, d.src_h, d.dst_h, true, d.src_w, d.dst_w);
+    return ws_layout(pl, d.src_h, d.src_h, d.dst_h, false, d.src_w, d.dst_w);
 }
 // One band of the sharded schedule.
 WsLayout ws_layout(const avirb200_plan* pl, const avirb200_shard_info& si) {
-    return ws_layout(pl, si.need_rows, si.src_rows, si.dst_rows, false, pl->desc.src_w, pl->desc.dst_w);
+    return ws_layout(pl, si.need_rows, si.src_rows, si.dst_rows, true, pl->desc.src_w, pl->desc.dst_w);
 }
 // A destination window of w columns and h rows with its footprint wi.
 WsLayout ws_layout(const avirb200_plan* pl, const avirb200_window_info& wi, int w, int h) {
-    return ws_layout(pl, wi.mid_rows, wi.src_h, h, true, wi.src_w, w);
+    return ws_layout(pl, wi.mid_rows, wi.src_h, h, false, wi.src_w, w);
+}
+
+// A double source's rows (cols pixels each) as floats into the workspace's in32: upstream's (float) cast.
+int narrow_source(const avirb200_plan* pl, const void* d_src, size_t src_pitch, int cols, int rows, float* in32,
+                  cudaStream_t st, int* launches) {
+    const int re = cols * pl->desc.channels;
+    const long long n = (long long)re * rows;
+    if (n == 0) return 0;
+    narrow_f64_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(static_cast<const double*>(d_src), (long long)src_pitch,
+                                                                   in32, re, rows);
+    ++*launches;
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
+// Where a band's ditherer takes the D row of its first row from and leaves the D row below its last (ErrdParams).
+struct ErrdCarry {
+    const float* in = nullptr;
+    const unsigned long long* in_prog = nullptr;
+    float* out = nullptr;
+    unsigned long long* out_prog = nullptr;
+    unsigned seq = 0;
+};
+
+// The column pass's float rows (out32: rows x cols pixels) into the caller's destination: widened to double,
+// or dithered (whole rows: cols is the image's width) with the boundary rows and counters at bnd / prog.
+int finish_rows(const avirb200_plan* pl, const float* out32, float* bnd, int* prog, int cols, int rows, void* d_dst,
+                size_t dst_pitch, const ErrdCarry& carry, cudaStream_t st, int* launches) {
+    const avirb200_plan_desc& d = pl->desc;
+    if (pl->io_out_type == AVIRB200_F64) {
+        const int re = cols * d.channels;
+        const long long n = (long long)re * rows;
+        if (n == 0) return 0;
+        widen_f32_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(out32, static_cast<double*>(d_dst),
+                                                                      (long long)dst_pitch, re, rows);
+        ++*launches;
+        CUDA_TRY(cudaGetLastError());
+    }
+    if (pl->errd) {
+        ErrdParams ep;
+        ep.src = out32;
+        ep.dst = d_dst;
+        ep.dst_pitch = (long long)dst_pitch;
+        ep.W = cols; ep.H = rows;
+        ep.dst_type = pl->io_out_type;
+        ep.round_mode = d.round_mode;
+        ep.planar = (d.sum_mode == AVIRB200_SUM_DIL8) ? 1 : 0;
+        ep.tr_mul = d.tr_mul; ep.tr_mul_inv = d.tr_mul_inv; ep.pk_out = d.pk_out;
+        ep.boundary = bnd;
+        ep.progress = prog;
+        ep.carry_in = carry.in; ep.carry_in_prog = carry.in_prog;
+        ep.carry_out = carry.out; ep.carry_out_prog = carry.out_prog;
+        ep.seq = carry.seq;
+        const int groups = errd_groups(rows);
+        CUDA_TRY(cudaMemsetAsync(prog, 0, (size_t)groups * 4, st));
+        switch (d.channels) {
+        case 1: errd_kernel<1><<<groups, 32, 0, st>>>(ep); break;
+        case 2: errd_kernel<2><<<groups, 32, 0, st>>>(ep); break;
+        case 3: errd_kernel<3><<<groups, 32, 0, st>>>(ep); break;
+        default: errd_kernel<4><<<groups, 32, 0, st>>>(ep); break;
+        }
+        ++*launches;
+        CUDA_TRY(cudaGetLastError());
+    }
+    return 0;
 }
 
 // ---- host-call staging: one set of device buffers per device, shared by every plan ----------------
@@ -852,24 +965,39 @@ int plan_staging(avirb200_plan* pl, size_t in_bytes, size_t out_bytes, size_t ws
 // Two slots (call parity): a rank can be at most one call ahead of a neighbour, because its
 // column pass needs that neighbour's rows of the same call.  avirb200_resize_sharded_local keeps
 // one mailbox per band in one device's memory, with one slot.
+// Error diffusion: band q-1's ditherer stores the D row below its last row into band q's mailbox with peer
+// stores and raises a progress word (call sequence number << 32 | pixels published); band q's ditherer waits
+// on it pixel by pixel.  The word names its call, so it is never reset (DESIGN.md section 7).
 //
 // The mailbox of band q, as MailboxLayout describes it:
-//   [256 B header: flag "from above" at +0, flag "from below" at +4, the sender's counters at +64]
-//   slot 0: [rows from q-1: halo_up(q)] [rows from q+1: halo_down(q), at +align256(up_bytes)]   slot 1: the same
+//   [256 B header: flag "from above" at +0, flag "from below" at +4, the sender's counters at +64,
+//    the error-diffusion progress words of slots 0 and 1 at +128 and +136]
+//   slot 0: [rows from q-1: halo_up(q)] [rows from q+1: halo_down(q), at +align256(up_bytes)]
+//           [error diffusion: D row from q-1, dst_w * channels floats, at +align256(up) + align256(down)]
+//   slot 1: the same
 struct MailboxLayout {
-    static constexpr size_t kHeader = 256, kCounters = 64;
-    size_t up_bytes = 0, down_bytes = 0;
+    static constexpr size_t kHeader = 256, kCounters = 64, kErrdProgress = 128;
+    size_t up_bytes = 0, down_bytes = 0, errd_bytes = 0;
     MailboxLayout() = default;
     MailboxLayout(const avirb200_plan* pl, const avirb200_shard_info& si)
         : up_bytes((size_t)si.halo_up * mid_pitch(pl) * sizeof(float)),
-          down_bytes((size_t)si.halo_down * mid_pitch(pl) * sizeof(float)) {}
-    size_t slot_bytes() const { return align_up(up_bytes, 256) + align_up(down_bytes, 256); }
+          down_bytes((size_t)si.halo_down * mid_pitch(pl) * sizeof(float)),
+          errd_bytes(pl->errd ? (size_t)pl->desc.dst_w * pl->desc.channels * sizeof(float) : 0) {}
+    size_t slot_bytes() const { return align_up(up_bytes, 256) + align_up(down_bytes, 256) + align_up(errd_bytes, 256); }
     size_t bytes(int slots) const { return kHeader + (size_t)slots * slot_bytes(); }
     // the mailbox at `box` (this process's address of it), slot `slot`
     avs::StreamMailbox at(char* box, int slot) const {
         char* s = box + kHeader + (size_t)slot * slot_bytes();
         return {reinterpret_cast<float*>(s), reinterpret_cast<float*>(s + align_up(up_bytes, 256)),
                 reinterpret_cast<unsigned*>(box), reinterpret_cast<unsigned long long*>(box + kCounters)};
+    }
+    // error diffusion: the D row from the band above and its progress word, slot `slot`
+    float* errd_row(char* box, int slot) const {
+        return reinterpret_cast<float*>(box + kHeader + (size_t)slot * slot_bytes() + align_up(up_bytes, 256) +
+                                        align_up(down_bytes, 256));
+    }
+    unsigned long long* errd_progress(char* box, int slot) const {
+        return reinterpret_cast<unsigned long long*>(box + kErrdProgress) + slot;
     }
 };
 
@@ -1079,7 +1207,24 @@ int sharded_push(avirb200_plan* pl, cudaStream_t st, const float* own, const avs
     return 0;
 }
 
-bool plan_has_f64(const avirb200_plan* pl) { // plans that only run as a whole image through resize_device / _host
+// Plans the banded host call runs unbanded: double buffers and error diffusion (bands on one compute stream would
+// restart the ditherer's wavefront once per band).
+// The plan's element types: the caller's (io_*), and what the kernels read and write (desc).
+void set_plan_types(avirb200_plan* pl, const avirb200_plan_desc* desc) {
+    pl->desc = *desc;
+    pl->io_in_type = desc->in_type;
+    pl->io_out_type = desc->out_type;
+    pl->mid_ch = desc->channels;
+    if (desc->in_type == AVIRB200_F64) pl->desc.in_type = AVIRB200_F32;   // cast on the device first
+    if (desc->out_type == AVIRB200_F64) pl->desc.out_type = AVIRB200_F32; // widened on the device last
+    if (desc->dither == 1 && (desc->out_type == AVIRB200_U8 || desc->out_type == AVIRB200_U16)) {
+        // the column pass delivers the gamma-corrected float rows; errd_kernel rounds them in row order
+        pl->errd = true;
+        pl->desc.out_type = AVIRB200_F32;
+    }
+}
+
+bool plan_has_f64(const avirb200_plan* pl) {
     return pl->io_in_type == AVIRB200_F64 || pl->io_out_type == AVIRB200_F64 || pl->errd;
 }
 
@@ -1186,15 +1331,8 @@ int avirb200_plan_create(const avirb200_plan_desc* desc, avirb200_plan** out) {
     }
     std::unique_ptr<avirb200_plan> pl(new (std::nothrow) avirb200_plan());
     if (!pl) return fail(AVIRB200_ERR_ALLOC, "host allocation failed");
-    pl->desc = *desc;
-    pl->io_in_type = desc->in_type;
-    pl->io_out_type = desc->out_type;
-    if (desc->in_type == AVIRB200_F64) pl->desc.in_type = AVIRB200_F32;   // cast on the device first
-    if (desc->out_type == AVIRB200_F64) pl->desc.out_type = AVIRB200_F32; // widened on the device last
-    if (desc->dither == 1 && (desc->out_type == AVIRB200_U8 || desc->out_type == AVIRB200_U16)) {
-        // the column pass delivers the gamma-corrected float rows; errd_kernel rounds them in row order
-        pl->errd = true;
-        pl->desc.out_type = AVIRB200_F32;
+    set_plan_types(pl.get(), desc);
+    if (pl->errd) {
         // errd_kernel's blocks (one warp per 32 rows) wait for their predecessor: keep all of them
         // resident at once (132 SMs x 32 blocks on an H100) instead of relying on in-order block dispatch
         // (32 one-warp blocks per SM; the SM count of the current device, where the plan will live)
@@ -1331,13 +1469,10 @@ int resize_region(const avirb200_plan* pl, const avirb200_window_info* win, int 
     void* kdst = d_dst;
     size_t kdst_pitch = dst_pitch;
     if (pl->io_in_type == AVIRB200_F64) {
-        const int re = src_w * d.channels;
-        const long long n = (long long)re * src_h;
-        narrow_f64_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(static_cast<const double*>(d_src),
-                                                                       (long long)src_pitch, in32, re, src_h);
-        ++launches;
+        const int e = narrow_source(pl, d_src, src_pitch, src_w, src_h, in32, st, &launches);
+        if (e != 0) return e;
         ksrc = in32;
-        ksrc_pitch = (size_t)re;
+        ksrc_pitch = (size_t)src_w * d.channels;
     }
     if (pl->io_out_type == AVIRB200_F64 || pl->errd) {
         kdst = out32;
@@ -1359,36 +1494,9 @@ int resize_region(const avirb200_plan* pl, const avirb200_window_info* win, int 
     col.scratch4 = wsb + ws.dst4;
     int r = run_pass(pl, row, st, &launches);
     if (r == 0) r = run_pass(pl, col, st, &launches);
-    if (r == 0 && pl->io_out_type == AVIRB200_F64) {
-        const int re = w * d.channels;
-        const long long n = (long long)re * h;
-        widen_f32_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(out32, static_cast<double*>(d_dst),
-                                                                      (long long)dst_pitch, re, h);
-        ++launches;
-        CUDA_TRY(cudaGetLastError());
-    }
-    if (r == 0 && pl->errd) {
-        ErrdParams ep;
-        ep.src = out32;
-        ep.dst = d_dst;
-        ep.dst_pitch = (long long)dst_pitch;
-        ep.W = d.dst_w; ep.H = d.dst_h;
-        ep.dst_type = pl->io_out_type;
-        ep.round_mode = d.round_mode;
-        ep.planar = (d.sum_mode == AVIRB200_SUM_DIL8) ? 1 : 0;
-        ep.tr_mul = d.tr_mul; ep.tr_mul_inv = d.tr_mul_inv; ep.pk_out = d.pk_out;
-        ep.boundary = reinterpret_cast<float*>(wsb + ws.errd_bnd);
-        ep.progress = reinterpret_cast<int*>(wsb + ws.errd_prog);
-        CUDA_TRY(cudaMemsetAsync(ep.progress, 0, (size_t)errd_groups(pl) * 4, st));
-        switch (d.channels) {
-        case 1: errd_kernel<1><<<errd_groups(pl), 32, 0, st>>>(ep); break;
-        case 2: errd_kernel<2><<<errd_groups(pl), 32, 0, st>>>(ep); break;
-        case 3: errd_kernel<3><<<errd_groups(pl), 32, 0, st>>>(ep); break;
-        default: errd_kernel<4><<<errd_groups(pl), 32, 0, st>>>(ep); break;
-        }
-        ++launches;
-        CUDA_TRY(cudaGetLastError());
-    }
+    if (r == 0)
+        r = finish_rows(pl, out32, reinterpret_cast<float*>(wsb + ws.errd_bnd), reinterpret_cast<int*>(wsb + ws.errd_prog), w,
+                        h, d_dst, dst_pitch, ErrdCarry(), st, &launches);
     pl->last_launches.store(launches, std::memory_order_relaxed);
     if (n_launches != nullptr) *n_launches = launches;
     return r;
@@ -1488,24 +1596,45 @@ int avirb200_row_pass_device(const avirb200_plan* pl, const void* d_src, size_t 
                              void* d_ws, void* stream) {
     if (pl == nullptr || d_src == nullptr || d_ws == nullptr)
         return fail(AVIRB200_ERR_BAD_ARG, "null argument");
-    if (plan_has_f64(pl)) return fail(AVIRB200_ERR_UNSUPPORTED, "per-pass entry points: no double buffers, no error diffusion");
+    const avirb200_plan_desc& d = pl->desc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const WsLayout ws = ws_layout(pl);
     int launches = 0;
-    PassRequest q = row_request(pl->desc, d_src, src_pitch, pl->desc.src_h, static_cast<float*>(d_ws), mid_pitch(pl));
-    q.scratch4 = static_cast<char*>(d_ws) + ws_layout(pl).src4;
-    return run_pass(pl, q, static_cast<cudaStream_t>(stream), &launches);
+    if (pl->io_in_type == AVIRB200_F64) { // the float copy of the source first, as resize_device makes it
+        if (src_pitch < (size_t)d.src_w * d.channels) return fail(AVIRB200_ERR_BAD_ARG, "pitch smaller than a row");
+        float* in32 = reinterpret_cast<float*>(static_cast<char*>(d_ws) + ws.in32);
+        const int e = narrow_source(pl, d_src, src_pitch, d.src_w, d.src_h, in32, st, &launches);
+        if (e != 0) return e;
+        d_src = in32;
+        src_pitch = (size_t)d.src_w * d.channels;
+    }
+    PassRequest q = row_request(d, d_src, src_pitch, d.src_h, static_cast<float*>(d_ws), mid_pitch(pl));
+    q.scratch4 = static_cast<char*>(d_ws) + ws.src4;
+    return run_pass(pl, q, st, &launches);
 }
 
 int avirb200_col_pass_device(const avirb200_plan* pl, const void* d_ws, void* d_dst,
                              size_t dst_pitch, void* stream) {
     if (pl == nullptr || d_dst == nullptr || d_ws == nullptr)
         return fail(AVIRB200_ERR_BAD_ARG, "null argument");
-    if (plan_has_f64(pl)) return fail(AVIRB200_ERR_UNSUPPORTED, "per-pass entry points: no double buffers, no error diffusion");
     const avirb200_plan_desc& d = pl->desc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    char* wsb = static_cast<char*>(const_cast<void*>(d_ws));
+    const WsLayout ws = ws_layout(pl);
     int launches = 0;
-    PassRequest q = col_request(d, d.dst_w, static_cast<const float*>(d_ws), mid_pitch(pl), 0, d.src_h, d_dst, dst_pitch,
+    // double output and error diffusion: the float rows into the workspace, then widened / dithered
+    const bool f32_out = pl->io_out_type == AVIRB200_F64 || pl->errd;
+    if (f32_out && dst_pitch < (size_t)d.dst_w * d.channels) return fail(AVIRB200_ERR_BAD_ARG, "pitch smaller than a row");
+    float* out32 = reinterpret_cast<float*>(wsb + ws.out32);
+    PassRequest q = col_request(d, d.dst_w, static_cast<const float*>(d_ws), mid_pitch(pl), 0, d.src_h,
+                                f32_out ? static_cast<void*>(out32) : d_dst, f32_out ? (size_t)d.dst_w * d.channels : dst_pitch,
                                 0, d.dst_h);
-    q.scratch4 = static_cast<char*>(const_cast<void*>(d_ws)) + ws_layout(pl).dst4;
-    return run_pass(pl, q, static_cast<cudaStream_t>(stream), &launches);
+    q.scratch4 = wsb + ws.dst4;
+    int r = run_pass(pl, q, st, &launches);
+    if (r == 0 && f32_out)
+        r = finish_rows(pl, out32, reinterpret_cast<float*>(wsb + ws.errd_bnd), reinterpret_cast<int*>(wsb + ws.errd_prog),
+                        d.dst_w, d.dst_h, d_dst, dst_pitch, ErrdCarry(), st, &launches);
+    return r;
 }
 
 int avirb200_resize_device_batch(const avirb200_plan* pl, int n, const void* const* d_srcs, size_t src_pitch,
@@ -1574,7 +1703,7 @@ int avirb200_resize_host(avirb200_plan* pl, const void* h_src, size_t src_pitch,
         const char* d1 = d0 + ((size_t)(d.dst_h - 1) * dst_pitch + (size_t)d.dst_w * d.channels) * out_el;
         if (s0 < d1 && d0 < s1) nb = 1;
     }
-    if (plan_has_f64(pl)) nb = 1; // the casts / the row-recursive ditherer run over the whole image
+    if (plan_has_f64(pl)) nb = 1; // the casts and the ditherer run over the whole image
     std::vector<avirb200_shard_info> si;
     while (nb >= 2) { // fewer bands until every band's column pass needs only its neighbours' rows
         si.assign(nb, avirb200_shard_info());
@@ -1732,6 +1861,28 @@ int avirb200_shard_workspace_bytes(const avirb200_plan* pl, int rank, int nranks
     return 0;
 }
 
+int avirb200_shard_layout_desc(const avirb200_plan_desc* desc, int rank, int nranks, size_t* ws_bytes,
+                               size_t* mailbox_bytes) {
+    if (desc == nullptr || ws_bytes == nullptr || mailbox_bytes == nullptr) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
+    if (desc->channels < 1 || desc->channels > 4 || desc->in_type < 0 || desc->in_type > 3 || desc->out_type < 0 ||
+        desc->out_type > 3)
+        return fail(AVIRB200_ERR_BAD_ARG, "bad image geometry or element type");
+    if (desc->v.nsteps < 1 || desc->v.nsteps > AVIRB200_MAX_STEPS)
+        return fail(AVIRB200_ERR_BAD_ARG, "axis: nsteps out of range");
+    // (host arithmetic on a plan that holds only its types: ws_layout and MailboxLayout read nothing else)
+    avirb200_plan pl;
+    set_plan_types(&pl, desc);
+    if (desc->channels < 4 && !plan_has_f64(&pl))
+        return fail(AVIRB200_ERR_UNSUPPORTED, "shard layout from a descriptor: a 1..3-channel plan may run widened "
+                                              "to 4 channels, which plan creation decides");
+    avirb200_shard_info si;
+    const int r = shard_compute_axis(host_axis_view(desc->v), rank, nranks, &si);
+    if (r != 0) return r;
+    *ws_bytes = ws_layout(&pl, si).total;
+    *mailbox_bytes = MailboxLayout(&pl, si).bytes(2);
+    return 0;
+}
+
 int avirb200_comm_unique_id(void* id128) {
     Nccl* nc = nccl();
     if (!nc) return fail(AVIRB200_ERR_NCCL, "libnccl.so.2 not loadable");
@@ -1759,7 +1910,6 @@ int avirb200_resize_sharded(const avirb200_plan* cpl, void* comm, int rank, int 
     if (cpl == nullptr || d_src == nullptr || d_dst == nullptr || d_ws == nullptr)
         return fail(AVIRB200_ERR_BAD_ARG, "null argument");
     avirb200_plan* pl = const_cast<avirb200_plan*>(cpl); // (exchange state is created on first use)
-    if (plan_has_f64(pl)) return fail(AVIRB200_ERR_UNSUPPORTED, "sharded calls: no double buffers, no error diffusion");
     { int cur = -1; if (cudaGetDevice(&cur) != cudaSuccess || cur != pl->device) return fail(AVIRB200_ERR_BAD_ARG, "the current device is not the plan's device"); }
     avirb200_shard_info si;
     int r = shard_compute(pl, rank, nranks, &si);
@@ -1771,19 +1921,38 @@ int avirb200_resize_sharded(const avirb200_plan* cpl, void* comm, int rank, int 
     float* mid = static_cast<float*>(d_ws);
     float* own = mid + (size_t)si.halo_up * rowf;
     const WsLayout ws = ws_layout(pl, si);
-    char* src4 = static_cast<char*>(d_ws) + ws.src4;
-    char* dst4 = static_cast<char*>(d_ws) + ws.dst4;
+    char* wsb = static_cast<char*>(d_ws);
+    char* src4 = wsb + ws.src4;
+    char* dst4 = wsb + ws.dst4;
     const size_t src4_row = (size_t)d.src_w * 4 * in_el;
     int launches = 0;
+    const bool f32_out = pl->io_out_type == AVIRB200_F64 || pl->errd;
+    if (f32_out && dst_pitch < (size_t)d.dst_w * d.channels) return fail(AVIRB200_ERR_BAD_ARG, "pitch smaller than a row");
+    // Double buffers: the band's source rows as floats first.  Double output and error diffusion: the column
+    // pass writes the band's float rows into the workspace, finish_rows() widens or dithers them last.
+    if (pl->io_in_type == AVIRB200_F64) {
+        if (src_pitch < (size_t)d.src_w * d.channels) return fail(AVIRB200_ERR_BAD_ARG, "pitch smaller than a row");
+        float* in32 = reinterpret_cast<float*>(wsb + ws.in32);
+        if ((r = narrow_source(pl, d_src, src_pitch, d.src_w, si.src_rows, in32, st, &launches)) != 0) return r;
+        d_src = in32;
+        src_pitch = (size_t)d.src_w * d.channels;
+    }
+    float* out32 = reinterpret_cast<float*>(wsb + ws.out32);
+    auto finish = [&](const ErrdCarry& cy) {
+        return finish_rows(pl, out32, reinterpret_cast<float*>(wsb + ws.errd_bnd), reinterpret_cast<int*>(wsb + ws.errd_prog),
+                           d.dst_w, si.dst_rows, d_dst, dst_pitch, cy, st, &launches);
+    };
     // the band's passes: its own rows into `own`, its destination rows from the intermediate rows it holds
     PassRequest row = row_request(d, d_src, src_pitch, si.src_rows, own, rowf);
     row.scratch4 = src4;
-    PassRequest col = col_request(d, d.dst_w, mid, rowf, si.need_row0, si.need_row0 + si.need_rows, d_dst, dst_pitch,
-                                  si.dst_row0, si.dst_row0 + si.dst_rows);
+    PassRequest col = col_request(d, d.dst_w, mid, rowf, si.need_row0, si.need_row0 + si.need_rows,
+                                  f32_out ? static_cast<void*>(out32) : d_dst,
+                                  f32_out ? (size_t)d.dst_w * d.channels : dst_pitch, si.dst_row0, si.dst_row0 + si.dst_rows);
     col.scratch4 = dst4;
     if (nranks <= 1) {
         r = run_pass(pl, row, st, &launches);
         if (r == 0) r = run_pass(pl, col, st, &launches);
+        if (r == 0 && f32_out) r = finish(ErrdCarry());
         pl->last_launches.store(launches, std::memory_order_relaxed);
         return r;
     }
@@ -1886,6 +2055,37 @@ int avirb200_resize_sharded(const avirb200_plan* cpl, void* comm, int rank, int 
             }
             r = run_pass(pl, col, st, &launches);
         }
+        // 5. double output: widened; error diffusion: the D row of the band above from this rank's mailbox, the
+        // band's own last D row into the mailbox of the rank below (peer stores), both in this call's slot
+        // Two slots hold because the sender's column pass of call n+1 waits for the receiver's rows of call n+1,
+        // which the receiver's stream produces after its ditherer of call n (DESIGN.md section 7).  A band that
+        // needs no rows from below (halo_down 0) has no such wait: its D row goes through NCCL instead.
+        if (r == 0 && f32_out) {
+            ErrdCarry cy;
+            cy.seq = seq;
+            float* carry = reinterpret_cast<float*>(wsb + ws.errd_carry);
+            const size_t rowd = (size_t)d.dst_w * d.channels;
+            const bool in_box = link.up && up.halo_down > 0, out_box = link.dn && si.halo_down > 0;
+            if (pl->errd && link.up) {
+                if (in_box) {
+                    cy.in = h->mine.errd_row(h->box, slot);
+                    cy.in_prog = h->mine.errd_progress(h->box, slot);
+                } else {
+                    NCCL_TRY(nc->Recv(carry, rowd, 7, rank - 1, comm, st));
+                    cy.in = carry;
+                }
+            }
+            if (pl->errd && link.dn) {
+                if (out_box) {
+                    cy.out = h->below.errd_row(h->box_down, slot);
+                    cy.out_prog = h->below.errd_progress(h->box_down, slot);
+                } else {
+                    cy.out = carry + rowd;
+                }
+            }
+            r = finish(cy);
+            if (r == 0 && pl->errd && link.dn && !out_box) NCCL_TRY(nc->Send(cy.out, rowd, 7, rank + 1, comm, st));
+        }
         // the pushes read this call's workspace: the caller's stream does not end before them
         if (pushed) CUDA_TRY(cudaStreamWaitEvent(st, pl->ev_x1, 0));
         pl->last_launches.store(launches, std::memory_order_relaxed);
@@ -1906,6 +2106,20 @@ int avirb200_resize_sharded(const avirb200_plan* cpl, void* comm, int rank, int 
     }
     NCCL_TRY(nc->GroupEnd());
     r = run_pass(pl, col, st, &launches);
+    // error diffusion: the D row of the band above arrives once rank-1's ditherer is done, this band's goes to
+    // rank+1 once its own is: the ranks' ditherers run one after another
+    if (r == 0 && f32_out) {
+        ErrdCarry cy;
+        float* carry = reinterpret_cast<float*>(wsb + ws.errd_carry);
+        const size_t rowd = (size_t)d.dst_w * d.channels;
+        if (pl->errd && rank > 0) {
+            NCCL_TRY(nc->Recv(carry, rowd, 7, rank - 1, comm, st));
+            cy.in = carry;
+        }
+        if (pl->errd && rank + 1 < nranks) cy.out = carry + rowd;
+        r = finish(cy);
+        if (r == 0 && cy.out != nullptr) NCCL_TRY(nc->Send(cy.out, rowd, 7, rank + 1, comm, st));
+    }
     pl->last_launches.store(launches, std::memory_order_relaxed);
     return r;
 }
@@ -1913,15 +2127,16 @@ int avirb200_resize_sharded(const avirb200_plan* cpl, void* comm, int rank, int 
 int avirb200_resize_sharded_host(avirb200_plan* pl, void* comm, int rank, int nranks, const void* h_src,
                                  size_t src_pitch, void* h_dst, size_t dst_pitch) {
     if (pl == nullptr || h_src == nullptr || h_dst == nullptr) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
-    if (plan_has_f64(pl)) return fail(AVIRB200_ERR_UNSUPPORTED, "sharded calls: no double buffers, no error diffusion");
     const avirb200_plan_desc& d = pl->desc;
     avirb200_shard_info si;
     int r = shard_compute(pl, rank, nranks, &si);
     if (r != 0) return r;
     size_t ws = 0;
     if ((r = avirb200_shard_workspace_bytes(pl, rank, nranks, &ws)) != 0) return r;
-    const size_t in_row = (size_t)d.src_w * d.channels * elem_size(d.in_type);
-    const size_t out_row = (size_t)d.dst_w * d.channels * elem_size(d.out_type);
+    // (the caller's element types: double bands are staged as doubles, dithered ones as integers)
+    const size_t in_el = elem_size(pl->io_in_type), out_el = elem_size(pl->io_out_type);
+    const size_t in_row = (size_t)d.src_w * d.channels * in_el;
+    const size_t out_row = (size_t)d.dst_w * d.channels * out_el;
     {
         std::lock_guard<std::mutex> lk(pl->mx);
         int cur = -1;
@@ -1932,12 +2147,12 @@ int avirb200_resize_sharded_host(avirb200_plan* pl, void* comm, int rank, int nr
     std::lock_guard<std::mutex> sl(staging_of(pl->device).mx);
     r = plan_staging(pl, in_row * si.src_rows, out_row * si.dst_rows, ws);
     if (r != 0) return r;
-    CUDA_TRY(cudaMemcpy2DAsync(pl->d_src, in_row, h_src, src_pitch * elem_size(d.in_type), in_row, si.src_rows,
+    CUDA_TRY(cudaMemcpy2DAsync(pl->d_src, in_row, h_src, src_pitch * in_el, in_row, si.src_rows,
                                cudaMemcpyHostToDevice, pl->stream));
     r = avirb200_resize_sharded(pl, comm, rank, nranks, pl->d_src, (size_t)d.src_w * d.channels, pl->d_dst,
                                 (size_t)d.dst_w * d.channels, pl->d_ws, pl->stream);
     if (r != 0) return r;
-    CUDA_TRY(cudaMemcpy2DAsync(h_dst, dst_pitch * elem_size(d.out_type), pl->d_dst, out_row, out_row, si.dst_rows,
+    CUDA_TRY(cudaMemcpy2DAsync(h_dst, dst_pitch * out_el, pl->d_dst, out_row, out_row, si.dst_rows,
                                cudaMemcpyDeviceToHost, pl->stream));
     CUDA_TRY(cudaStreamSynchronize(pl->stream));
     return 0;
@@ -1948,56 +2163,103 @@ int avirb200_resize_sharded_local(const avirb200_plan* pl, int nranks, const voi
                                   void* stream) {
     if (pl == nullptr || d_src == nullptr || d_dst == nullptr || d_ws == nullptr)
         return fail(AVIRB200_ERR_BAD_ARG, "null argument");
-    if (plan_has_f64(pl)) return fail(AVIRB200_ERR_UNSUPPORTED, "sharded calls: no double buffers, no error diffusion");
     const avirb200_plan_desc& d = pl->desc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const size_t rowf = mid_pitch(pl);
-    const size_t in_el = elem_size(d.in_type), out_el = elem_size(d.out_type);
+    // (the caller's element types; the kernels' source is the band's float copy when it is double)
+    const size_t in_el = elem_size(pl->io_in_type), out_el = elem_size(pl->io_out_type);
+    const bool f64_in = pl->io_in_type == AVIRB200_F64, f32_out = pl->io_out_type == AVIRB200_F64 || pl->errd;
+    if ((f64_in && src_pitch < (size_t)d.src_w * d.channels) || (f32_out && dst_pitch < (size_t)d.dst_w * d.channels))
+        return fail(AVIRB200_ERR_BAD_ARG, "pitch smaller than a row");
     std::vector<avirb200_shard_info> si(nranks);
     std::vector<float*> mid(nranks), own(nranks);
     std::vector<PassRequest> row(nranks), col(nranks);
+    std::vector<WsLayout> wsl(nranks);
+    std::vector<char*> wsb(nranks);
     char* base = static_cast<char*>(d_ws);
     for (int r = 0; r < nranks; ++r) { // every band's segment: as avirb200_shard_workspace_bytes lays it out
         int e = shard_compute(pl, r, nranks, &si[r]);
         if (e != 0) return e;
-        const WsLayout ws = ws_layout(pl, si[r]);
+        const WsLayout ws = wsl[r] = ws_layout(pl, si[r]);
+        wsb[r] = base;
         mid[r] = reinterpret_cast<float*>(base);
         own[r] = mid[r] + (size_t)si[r].halo_up * rowf;
-        row[r] = row_request(d, static_cast<const char*>(d_src) + (size_t)si[r].src_row0 * src_pitch * in_el, src_pitch,
-                             si[r].src_rows, own[r], rowf);
+        const char* band_src = static_cast<const char*>(d_src) + (size_t)si[r].src_row0 * src_pitch * in_el;
+        char* band_dst = static_cast<char*>(d_dst) + (size_t)si[r].dst_row0 * dst_pitch * out_el;
+        row[r] = f64_in ? row_request(d, base + ws.in32, (size_t)d.src_w * d.channels, si[r].src_rows, own[r], rowf)
+                        : row_request(d, band_src, src_pitch, si[r].src_rows, own[r], rowf);
         row[r].scratch4 = base + ws.src4;
         col[r] = col_request(d, d.dst_w, mid[r], rowf, si[r].need_row0, si[r].need_row0 + si[r].need_rows,
-                             static_cast<char*>(d_dst) + (size_t)si[r].dst_row0 * dst_pitch * out_el, dst_pitch,
+                             f32_out ? base + ws.out32 : band_dst, f32_out ? (size_t)d.dst_w * d.channels : dst_pitch,
                              si[r].dst_row0, si[r].dst_row0 + si[r].dst_rows);
         col[r].scratch4 = base + ws.dst4;
         base += ws.total;
     }
     int launches = 0;
+    // double buffers: every band's source rows as floats (upstream's cast), before the row passes
+    for (int r = 0; r < nranks && f64_in; ++r) {
+        const int e = narrow_source(pl, static_cast<const char*>(d_src) + (size_t)si[r].src_row0 * src_pitch * in_el,
+                                    src_pitch, d.src_w, si[r].src_rows, reinterpret_cast<float*>(wsb[r] + wsl[r].in32), st,
+                                    &launches);
+        if (e != 0) return e;
+    }
     // The fused halo exchange of avirb200_resize_sharded (AVIRB200_OPT_OVERLAP_HALO = 3), with every band's
     // mailbox (one slot) in this device's memory: the same two kernels, parameters and protocol as between
     // ranks.  Only when every band may run both fused halves and both its passes run on the streaming kernel.
+    // Error diffusion hands each band's last D row to the next band through the same mailboxes on every
+    // schedule (the bands' ditherers run in stream order: no wait ever spins).
     std::vector<avs::StreamLink> link(nranks);
     std::vector<MailboxLayout> box(nranks);
     std::vector<size_t> box_off(nranks + 1, 0);
     bool fused = pl->opt_overlap == 3 && nranks > 1;
-    for (int r = 0; r < nranks && fused; ++r) {
+    for (int r = 0; r < nranks; ++r) {
         link[r].me = &si[r];
         if (r > 0) link[r].up = &si[r - 1];
         if (r + 1 < nranks) link[r].dn = &si[r + 1];
-        fused = avs::stream_fused_tx_ok(link[r]) && pass_family(pl, row[r]).family == kFamilyStream &&
+        fused = fused && avs::stream_fused_tx_ok(link[r]) && pass_family(pl, row[r]).family == kFamilyStream &&
                 pass_family(pl, col[r]).family == kFamilyStream;
         box[r] = MailboxLayout(pl, si[r]);
         box_off[r + 1] = box_off[r] + box[r].bytes(1);
     }
-    if (fused) {
-        char* boxes = nullptr;
+    // the bands' float rows into the destination: widened, or dithered with the D row carried band to band
+    auto finish_bands = [&](char* boxes) -> int {
+        for (int r = 0; r < nranks && f32_out; ++r) {
+            ErrdCarry cy;
+            cy.seq = 1; // (the mailboxes are this call's own)
+            if (pl->errd && r > 0) {
+                cy.in = box[r].errd_row(boxes + box_off[r], 0);
+                cy.in_prog = box[r].errd_progress(boxes + box_off[r], 0);
+            }
+            if (pl->errd && r + 1 < nranks) {
+                cy.out = box[r + 1].errd_row(boxes + box_off[r + 1], 0);
+                cy.out_prog = box[r + 1].errd_progress(boxes + box_off[r + 1], 0);
+            }
+            const int e = finish_rows(pl, reinterpret_cast<const float*>(wsb[r] + wsl[r].out32),
+                                      reinterpret_cast<float*>(wsb[r] + wsl[r].errd_bnd),
+                                      reinterpret_cast<int*>(wsb[r] + wsl[r].errd_prog), d.dst_w, si[r].dst_rows,
+                                      static_cast<char*>(d_dst) + (size_t)si[r].dst_row0 * dst_pitch * out_el, dst_pitch,
+                                      cy, st, &launches);
+            if (e != 0) return e;
+        }
+        return 0;
+    };
+    char* boxes = nullptr;
+    if (fused || (pl->errd && nranks > 1)) {
         CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&boxes), box_off[nranks], st));
+        int e = 0;
+        for (int r = 0; r < nranks && e == 0; ++r)
+            if (cudaMemsetAsync(boxes + box_off[r], 0, MailboxLayout::kHeader, st) != cudaSuccess)
+                e = fail(AVIRB200_ERR_CUDA, "sharded_local: mailbox header");
+        if (e != 0) {
+            cudaFreeAsync(boxes, st);
+            return e;
+        }
+    }
+    if (fused) {
         int e = 0;
         for (int r = 0; r < nranks; ++r) {
             link[r].mine = box[r].at(boxes + box_off[r], 0);
             link[r].seq = 1;
-            if (e == 0 && cudaMemsetAsync(boxes + box_off[r], 0, MailboxLayout::kHeader, st) != cudaSuccess)
-                e = fail(AVIRB200_ERR_CUDA, "sharded_local: mailbox header");
         }
         for (int r = 0; r < nranks; ++r) {
             if (r > 0) link[r].above = link[r - 1].mine;
@@ -2007,10 +2269,16 @@ int avirb200_resize_sharded_local(const avirb200_plan* pl, int nranks, const voi
         }
         for (int r = 0; r < nranks && e == 0; ++r) e = run_pass(pl, row[r], st, &launches);
         for (int r = 0; r < nranks && e == 0; ++r) e = run_pass(pl, col[r], st, &launches);
+        if (e == 0) e = finish_bands(boxes);
         cudaFreeAsync(boxes, st);
         pl->last_launches.store(launches, std::memory_order_relaxed);
         return e;
     }
+    // (error diffusion: the mailboxes are released on every exit below)
+    struct BoxGuard {
+        char* p; cudaStream_t st;
+        ~BoxGuard() { if (p != nullptr) cudaFreeAsync(p, st); }
+    } box_guard{boxes, st};
     for (int r = 0; r < nranks; ++r) { // every band's row pass
         int e = run_pass(pl, row[r], st, &launches);
         if (e != 0) return e;
@@ -2030,6 +2298,7 @@ int avirb200_resize_sharded_local(const avirb200_plan* pl, int nranks, const voi
         int e = run_pass(pl, col[r], st, &launches);
         if (e != 0) return e;
     }
+    if (const int e = finish_bands(boxes)) return e;
     pl->last_launches.store(launches, std::memory_order_relaxed);
     return 0;
 }

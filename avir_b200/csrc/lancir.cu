@@ -40,6 +40,7 @@
 
 #include "avirb200.h"
 #include "host_util.h"
+#include "peer_mailbox.h"
 
 using avb::elem_size;
 using avb::fail;
@@ -229,21 +230,18 @@ constexpr int kLColRows = 32; // output rows a block of the column pass walks
 
 // KL: compile-time kernel length (all taps' loads of an output are issued before the first
 // product: the loop is unrolled) for the common lengths, 0 = run-time length.
-template <typename TIN, int KL>
-__global__ void __launch_bounds__(256) lancir_col4_kernel(const __grid_constant__ LParams p) {
-    const int px = blockIdx.x * 256 + threadIdx.x;
-    if (px >= p.mid_w) return;
-    const int y0 = blockIdx.y * kLColRows;
-    const int y1 = (y0 + kLColRows < p.win_h) ? y0 + kLColRows : p.win_h;
-    const int kl = KL ? KL : p.v.kl, src_h = p.src_h, fy0 = p.fy0;
-    const long long pitch = p.src_pitch;
+// The column pass of output rows [y0, y1) of the region for pixel px; row(sy, e) loads the 4 elements at e of
+// source row sy (clamped to the image).
+template <typename TIN, int KL, class Row>
+__device__ __forceinline__ void lcol4_rows(const LParams& p, const int px, const int y0, const int y1, Row row) {
+    const int kl = KL ? KL : p.v.kl, src_h = p.src_h;
     for (int y = y0; y < y1; ++y) {
         const float* f = p.v.taps + (size_t)__ldg(p.v.phase + p.y0 + y) * kl;
         const int s0 = __ldg(p.v.src_pos + p.y0 + y);
         auto S = [&](int t) {
             int sy = s0 + t;
             sy = sy < 0 ? 0 : (sy >= src_h ? src_h - 1 : sy);
-            return LPix<TIN>::load(p.src, (long long)(sy - fy0) * pitch + (long long)px * 4);
+            return row(sy, (long long)px * 4);
         };
         float4 ev, od;
         if (KL) {
@@ -265,6 +263,130 @@ __global__ void __launch_bounds__(256) lancir_col4_kernel(const __grid_constant_
         }
         reinterpret_cast<float4*>(p.mid + (size_t)y * p.mid_w * 4)[px] = ladd4(ev, od);
     }
+}
+
+// KL: compile-time kernel length (all taps' loads of an output are issued before the first
+// product: the loop is unrolled) for the common lengths, 0 = run-time length.
+template <typename TIN, int KL>
+__global__ void __launch_bounds__(256) lancir_col4_kernel(const __grid_constant__ LParams p) {
+    const int px = blockIdx.x * 256 + threadIdx.x;
+    if (px >= p.mid_w) return;
+    const int y0 = blockIdx.y * kLColRows;
+    const int y1 = (y0 + kLColRows < p.win_h) ? y0 + kLColRows : p.win_h;
+    const int fy0 = p.fy0;
+    const long long pitch = p.src_pitch;
+    lcol4_rows<TIN, KL>(p, px, y0, y1, [&](int sy, long long e) {
+        return LPix<TIN>::load(p.src, (long long)(sy - fy0) * pitch + e);
+    });
+}
+
+// ---- row-sharded calls: the column pass over a source in three segments ---------------------------
+// A band's column pass reads source rows [up0, row0) from the segment "from above" (the rank above's last
+// rows), its own band [row0, row0 + rows) from the caller's buffer (LParams src / src_pitch, fy0 = row0) and
+// the rows after it from the segment "from below".  Taps clamp to the image first, as everywhere.  A segment
+// with a flag is a peer mailbox: a block whose rows' taps reach it waits until the flag holds the call's
+// sequence number (the rows arrive before the flag, lancirb200_resize_sharded); a segment without one is
+// already in place (NCCL, device copies).  Picking a segment per tap costs registers, so the segmented kernels
+// run only a band's EDGE rows, [0, top) and [bot0, win_h): the rows whose taps reach beyond the band.  The
+// rows between read the band alone and run on the plain kernels (lancir_region).
+struct LSeg {
+    const void* up; long long up_pitch; // pitches in elements
+    const void* dn; long long dn_pitch;
+    int up0, row0, rows;
+    const volatile unsigned* flag_up;
+    const volatile unsigned* flag_dn;
+    unsigned seq;
+    int top, bot0;
+};
+
+__device__ __forceinline__ const void* lseg_row(const LParams& p, const LSeg& s, int sy, long long* off) {
+    if (sy < s.row0) {
+        *off = (long long)(sy - s.up0) * s.up_pitch;
+        return s.up;
+    }
+    if (sy >= s.row0 + s.rows) {
+        *off = (long long)(sy - s.row0 - s.rows) * s.dn_pitch;
+        return s.dn;
+    }
+    *off = (long long)(sy - s.row0) * p.src_pitch;
+    return p.src;
+}
+
+__device__ __forceinline__ void lseg_spin(const volatile unsigned* flag, unsigned seq) {
+    long long spins = 0;
+    while ((int)(*flag - seq) < 0) {
+        if (++spins > (1ll << 31)) __trap(); // a neighbour never delivered: fail instead of hanging
+        __nanosleep(100);
+    }
+    __threadfence_system();
+}
+
+// Every thread of the block calls it: the block's output rows [y0, y1) wait for the mailbox segments
+// their taps reach (the span of their clamped taps, as lspan computes it on the host).
+__device__ __forceinline__ void lseg_wait(const LParams& p, const LSeg& s, int y0, int y1) {
+    if (threadIdx.x == 0 && (s.flag_up || s.flag_dn)) {
+        const int kl = p.v.kl, src_h = p.src_h;
+        int lo = src_h, hi = -1;
+        for (int y = y0; y < y1; ++y) {
+            const int s0 = __ldg(p.v.src_pos + p.y0 + y);
+            const int a = s0 < 0 ? 0 : (s0 >= src_h ? src_h - 1 : s0);
+            const int b = s0 + kl - 1 < 0 ? 0 : (s0 + kl - 1 >= src_h ? src_h - 1 : s0 + kl - 1);
+            lo = a < lo ? a : lo;
+            hi = b > hi ? b : hi;
+        }
+        if (s.flag_up && lo < s.row0) lseg_spin(s.flag_up, s.seq);
+        if (s.flag_dn && hi >= s.row0 + s.rows) lseg_spin(s.flag_dn, s.seq);
+    }
+    __syncthreads();
+}
+
+// The rows [*y0, *y1) of row group blockIdx.y: groups of G rows over [0, top), then over [bot0, win_h).
+template <int G>
+__device__ __forceinline__ void lseg_rows(const LParams& p, const LSeg& s, int* y0, int* y1) {
+    const int gt = (s.top + G - 1) / G, g = (int)blockIdx.y;
+    const int a = g < gt ? g * G : s.bot0 + (g - gt) * G;
+    const int e = g < gt ? s.top : p.win_h;
+    *y0 = a;
+    *y1 = a + G < e ? a + G : e;
+}
+
+// lancir_col_kernel over a segmented source
+__global__ void __launch_bounds__(256) lancir_col_seg_kernel(const __grid_constant__ LParams p,
+                                                             const __grid_constant__ LSeg s) {
+    int y, y1;
+    lseg_rows<1>(p, s, &y, &y1);
+    lseg_wait(p, s, y, y1);
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    const int row_elems = p.mid_w * p.C;
+    if (e >= row_elems) return;
+    const int kl = p.v.kl;
+    const float* f = p.v.taps + (size_t)__ldg(p.v.phase + p.y0 + y) * kl;
+    const int s0 = __ldg(p.v.src_pos + p.y0 + y);
+    const int in_type = p.in_type, src_h = p.src_h;
+    const float r = ltapsum(p.C, e % p.C, kl, f, [&](int t) {
+        int sy = s0 + t;
+        sy = sy < 0 ? 0 : (sy >= src_h ? src_h - 1 : sy);
+        long long off;
+        const void* b = lseg_row(p, s, sy, &off);
+        return lload(b, in_type, off + e);
+    });
+    p.mid[(size_t)y * row_elems + e] = r;
+}
+
+// lancir_col4_kernel over a segmented source (every segment's pixels aligned to their size)
+template <typename TIN, int KL>
+__global__ void __launch_bounds__(256) lancir_col4_seg_kernel(const __grid_constant__ LParams p,
+                                                              const __grid_constant__ LSeg s) {
+    int y0, y1;
+    lseg_rows<kLColRows>(p, s, &y0, &y1);
+    lseg_wait(p, s, y0, y1);
+    const int px = blockIdx.x * 256 + threadIdx.x;
+    if (px >= p.mid_w) return;
+    lcol4_rows<TIN, KL>(p, px, y0, y1, [&](int sy, long long e) {
+        long long off;
+        const void* b = lseg_row(p, s, sy, &off);
+        return LPix<TIN>::load(b, off + e);
+    });
 }
 
 // OUT: 0 float, 1 u8, 2 u16, 3 double, 4 uint32_t
@@ -354,6 +476,77 @@ int lwindow(const int32_t* hpos, int hkl, const int32_t* vpos, int vkl, int src_
     return 0;
 }
 
+// Row-sharded calls: the bands of rank `rank` of `nranks`, by AVIR's partition rule (source rows src_h * r / n,
+// destination rows dst_h * r / n).  need_* are SOURCE rows: the band's vertical footprint (lspan) joined with
+// its own source band; the halos are the rows of it beyond the band, which the neighbours hold.
+int lshard(const int32_t* vpos, int vkl, int src_h, int dst_h, int rank, int nranks, avirb200_shard_info* info) {
+    if (nranks < 1 || rank < 0 || rank >= nranks) return fail(AVIRB200_ERR_BAD_ARG, "bad rank");
+    auto src_split = [&](int r) { return (int)((long long)src_h * r / nranks); };
+    auto dst_split = [&](int r) { return (int)((long long)dst_h * r / nranks); };
+    info->src_row0 = src_split(rank);
+    info->src_rows = src_split(rank + 1) - info->src_row0;
+    info->dst_row0 = dst_split(rank);
+    info->dst_rows = dst_split(rank + 1) - info->dst_row0;
+    if (info->dst_rows <= 0 || info->src_rows <= 0) return fail(AVIRB200_ERR_UNSUPPORTED, "image has fewer rows than ranks");
+    if (info->dst_rows > 65535) return fail(AVIRB200_ERR_UNSUPPORTED, "band too tall (more than 65535 destination rows)");
+    int32_t lo = 0, n = 0;
+    lspan(vpos, vkl, src_h, info->dst_row0, info->dst_rows, &lo, &n);
+    const int a = lo < info->src_row0 ? lo : info->src_row0;
+    const int b = lo + n > info->src_row0 + info->src_rows ? lo + n : info->src_row0 + info->src_rows;
+    info->need_row0 = a;
+    info->need_rows = b - a;
+    info->halo_up = info->src_row0 - a;
+    info->halo_down = b - (info->src_row0 + info->src_rows);
+    if (rank > 0 && info->halo_up > info->src_row0 - src_split(rank - 1))
+        return fail(AVIRB200_ERR_UNSUPPORTED, "halo exceeds the neighbouring band (too many ranks)");
+    if (rank + 1 < nranks && info->halo_down > src_split(rank + 2) - src_split(rank + 1))
+        return fail(AVIRB200_ERR_UNSUPPORTED, "halo exceeds the neighbouring band (too many ranks)");
+    return 0;
+}
+
+// Bytes of one source row in a halo segment: 16-byte aligned, so that the vector kernel's loads stay aligned.
+size_t lhalo_row_bytes(const lancirb200_plan_desc& d) {
+    return avb::align_up((size_t)d.src_w * d.channels * elem_size(d.in_type), 16);
+}
+
+// A band's workspace: [intermediate: dst_rows x src_w x C floats] [rows from above: halo_up rows]
+// [rows from below: halo_down rows] [header: the flags lancirb200_resize_sharded_local raises], each part
+// 256-byte aligned.  The halo segments receive the neighbours' rows on the NCCL schedule.
+struct LShardWs {
+    static constexpr size_t kHeader = 256;
+    size_t up = 0, down = 0, header = 0, total = 0;
+    LShardWs(const lancirb200_plan_desc& d, const avirb200_shard_info& si) {
+        const size_t row = lhalo_row_bytes(d);
+        up = avb::align_up((size_t)si.dst_rows * d.src_w * d.channels * sizeof(float), 256);
+        down = up + avb::align_up((size_t)si.halo_up * row, 256);
+        header = down + avb::align_up((size_t)si.halo_down * row, 256);
+        total = header + kHeader;
+    }
+};
+
+// A rank's mailbox: [256 B header: flag "from above" at +0, flag "from below" at +4]
+//   slot 0: [rows from rank-1: halo_up rows] [rows from rank+1: halo_down rows, at +align256(up_bytes)]
+//   slot 1: the same
+// Rows lhalo_row_bytes apart, in the caller's element type.
+struct LBoxLayout {
+    static constexpr size_t kHeader = 256;
+    size_t up_bytes = 0, down_bytes = 0;
+    LBoxLayout() = default;
+    LBoxLayout(const lancirb200_plan_desc& d, const avirb200_shard_info& si)
+        : up_bytes((size_t)si.halo_up * lhalo_row_bytes(d)), down_bytes((size_t)si.halo_down * lhalo_row_bytes(d)) {}
+    size_t slot_bytes() const { return avb::align_up(up_bytes, 256) + avb::align_up(down_bytes, 256); }
+    size_t bytes(int slots) const { return kHeader + (size_t)slots * slot_bytes(); }
+    char* from_up(char* box, int slot) const { return box + kHeader + (size_t)slot * slot_bytes(); }
+    char* from_down(char* box, int slot) const { return from_up(box, slot) + avb::align_up(up_bytes, 256); }
+};
+
+struct LHalo : avb::PeerBoxes {
+    void* comm = nullptr;
+    int rank = -1, nranks = 0;
+    LBoxLayout mine, above, below;
+    unsigned seq = 0;
+};
+
 } // namespace
 
 struct lancirb200_plan {
@@ -368,6 +561,12 @@ struct lancirb200_plan {
     void* d_ws = nullptr;
     size_t src_bytes = 0, dst_bytes = 0, ws_bytes = 0;
     cudaStream_t stream = nullptr;
+    // row-sharded calls
+    int opt_overlap = 3;           // AVIRB200_OPT_OVERLAP_HALO: 3 mailboxes, 0 NCCL
+    LHalo* halo = nullptr;         // the peer mailboxes (created by the first sharded call)
+    unsigned* h_one = nullptr;     // pinned 1: the flag value of lancirb200_resize_sharded_local
+    cudaStream_t stream_x = nullptr; // exchange stream
+    cudaEvent_t ev_x0 = nullptr, ev_x1 = nullptr;
 };
 
 extern "C" {
@@ -436,6 +635,14 @@ void lancirb200_plan_destroy(lancirb200_plan* pl) {
     if (!pl) return;
     cudaFree(pl->arena); cudaFree(pl->d_src); cudaFree(pl->d_dst); cudaFree(pl->d_ws);
     if (pl->stream) cudaStreamDestroy(pl->stream);
+    if (pl->halo) {
+        avb::peer_boxes_close(pl->halo);
+        delete pl->halo;
+    }
+    cudaFreeHost(pl->h_one);
+    if (pl->stream_x) cudaStreamDestroy(pl->stream_x);
+    if (pl->ev_x0) cudaEventDestroy(pl->ev_x0);
+    if (pl->ev_x1) cudaEventDestroy(pl->ev_x1);
     delete pl;
 }
 
@@ -450,9 +657,11 @@ int lancirb200_plan_workspace_bytes(const lancirb200_plan* pl, size_t* bytes) {
 namespace {
 
 // Both passes over the destination region [x0, x0 + w) x [y0, y0 + h): d_src holds the source from row fy0
-// on, its column 0 is source column fx0, and the intermediate in d_ws is h rows of fw pixels.
+// on, its column 0 is source column fx0, and the intermediate in d_ws is h rows of fw pixels.  seg: the
+// column pass reads a segmented source (row-sharded calls; fy0 is then the band's first row).
 int lancir_region(const lancirb200_plan* pl, int x0, int y0, int w, int h, int fx0, int fw, int fy0,
-                  const void* d_src, size_t src_pitch, void* d_dst, size_t dst_pitch, void* d_ws, void* stream) {
+                  const void* d_src, size_t src_pitch, void* d_dst, size_t dst_pitch, void* d_ws, void* stream,
+                  const LSeg* seg = nullptr) {
     const lancirb200_plan_desc& d = pl->desc;
     LParams p;
     p.v = pl->dv; p.h = pl->dh;
@@ -467,20 +676,39 @@ int lancir_region(const lancirb200_plan* pl, int x0, int y0, int w, int h, int f
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     if (h > 65535) return fail(AVIRB200_ERR_UNSUPPORTED, "image too tall");
     (void)cudaGetLastError(); // (a stale non-sticky error of another library is not this launch's)
-    // 4-channel images whose pixels are aligned to their own size: the vector kernels
+    // 4-channel images whose pixels are aligned to their own size: the vector kernels (a segmented source's
+    // halo segments are aligned by construction)
     const bool vec_in = d.channels == 4 && (src_pitch % 4) == 0 && ((uintptr_t)d_src % (4 * elem_size(d.in_type))) == 0 &&
                         ((uintptr_t)d_ws % 16) == 0;
     const bool vec_out = d.channels == 4 && (dst_pitch % 4) == 0 && ((uintptr_t)d_dst % (4 * elem_size(d.out_type))) == 0 &&
                          ((uintptr_t)d_ws % 16) == 0;
+    // a band (seg): the plain kernel over its interior rows [top, bot0), the segmented one over its edge rows
+    LParams pi = p;
+    LSeg s;
+    std::memset(&s, 0, sizeof s);
+    int ni = h, ne = 0; // interior rows, edge row groups
+    if (seg) {
+        s = *seg;
+        pi.y0 += s.top;
+        pi.win_h = ni = s.bot0 - s.top;
+        pi.mid += (size_t)s.top * fw * d.channels;
+    }
     if (vec_in) {
-        dim3 g1((fw + 255) / 256, (h + kLColRows - 1) / kLColRows);
+        auto groups = [](int rows) { return (rows + kLColRows - 1) / kLColRows; };
+        if (seg) ne = groups(s.top) + groups(h - s.bot0);
+        const dim3 g1((fw + 255) / 256, groups(ni)), ge((fw + 255) / 256, ne);
+#define LCOL1(T, KL)                                                                                    \
+    do {                                                                                                \
+        if (ni > 0) lancir_col4_kernel<T, KL><<<g1, 256, 0, st>>>(pi);                                  \
+        if (ne > 0) lancir_col4_seg_kernel<T, KL><<<ge, 256, 0, st>>>(p, s);                            \
+    } while (0)
 #define LCOL(KL)                                                                                        \
     do {                                                                                                \
-        if (d.in_type == AVIRB200_U8) lancir_col4_kernel<unsigned char, KL><<<g1, 256, 0, st>>>(p);     \
-        else if (d.in_type == AVIRB200_U16) lancir_col4_kernel<unsigned short, KL><<<g1, 256, 0, st>>>(p); \
-        else if (d.in_type == AVIRB200_F64) lancir_col4_kernel<double, KL><<<g1, 256, 0, st>>>(p);      \
-        else if (d.in_type == AVIRB200_U32) lancir_col4_kernel<unsigned int, KL><<<g1, 256, 0, st>>>(p); \
-        else lancir_col4_kernel<float, KL><<<g1, 256, 0, st>>>(p);                                      \
+        if (d.in_type == AVIRB200_U8) LCOL1(unsigned char, KL);                                         \
+        else if (d.in_type == AVIRB200_U16) LCOL1(unsigned short, KL);                                  \
+        else if (d.in_type == AVIRB200_F64) LCOL1(double, KL);                                          \
+        else if (d.in_type == AVIRB200_U32) LCOL1(unsigned int, KL);                                    \
+        else LCOL1(float, KL);                                                                          \
     } while (0)
         switch (pl->dv.kl) { // la = 3: 6 taps when upsizing, 12 at k = 2, 18 at k = 3, 24 at k = 4
         case 6: LCOL(6); break;
@@ -490,9 +718,12 @@ int lancir_region(const lancirb200_plan* pl, int x0, int y0, int w, int h, int f
         default: LCOL(0); break;
         }
 #undef LCOL
+#undef LCOL1
     } else {
-        dim3 g1((fw * d.channels + 255) / 256, h);
-        lancir_col_kernel<<<g1, 256, 0, st>>>(p);
+        if (seg) ne = s.top + (h - s.bot0);
+        const dim3 g1((fw * d.channels + 255) / 256, ni), ge((fw * d.channels + 255) / 256, ne);
+        if (ni > 0) lancir_col_kernel<<<g1, 256, 0, st>>>(pi);
+        if (ne > 0) lancir_col_seg_kernel<<<ge, 256, 0, st>>>(p, s);
     }
     if (vec_out) {
         dim3 g2((w + 255) / 256, h);
@@ -670,6 +901,335 @@ int lancirb200_resize_window_host(lancirb200_plan* pl, int x0, int y0, int w, in
                                pl->stream));
     CUDA_TRY(cudaStreamSynchronize(pl->stream));
     return 0;
+}
+
+} // extern "C"
+
+// ---- row-sharded calls ---------------------------------------------------------------------------
+
+namespace {
+
+int lshard_plan(const lancirb200_plan* pl, int rank, int nranks, avirb200_shard_info* si) {
+    const lancirb200_plan_desc& d = pl->desc;
+    return lshard(pl->pos_v.data(), pl->dv.kl, d.src_h, d.dst_h, rank, nranks, si);
+}
+
+int lgrow(void** p, size_t* have, size_t need) {
+    if (*have >= need) return 0;
+    cudaFree(*p);
+    *p = nullptr; *have = 0;
+    CUDA_TRY(cudaMalloc(p, need));
+    *have = need;
+    return 0;
+}
+
+// The exchange stream, forked from `st` (it starts after everything enqueued on st so far).
+int lfork(lancirb200_plan* pl, cudaStream_t st) {
+    if (pl->stream_x == nullptr) CUDA_TRY(cudaStreamCreateWithFlags(&pl->stream_x, cudaStreamNonBlocking));
+    if (pl->ev_x0 == nullptr) CUDA_TRY(cudaEventCreateWithFlags(&pl->ev_x0, cudaEventDisableTiming));
+    if (pl->ev_x1 == nullptr) CUDA_TRY(cudaEventCreateWithFlags(&pl->ev_x1, cudaEventDisableTiming));
+    CUDA_TRY(cudaEventRecord(pl->ev_x0, st));
+    CUDA_TRY(cudaStreamWaitEvent(pl->stream_x, pl->ev_x0, 0));
+    return 0;
+}
+
+// `n` source rows of a band from its row `r0` into a halo segment (rows lhalo_row_bytes apart), on `st`.
+int lcopy_rows(const lancirb200_plan* pl, void* seg, const void* band, size_t src_pitch, int r0, int n, cudaStream_t st) {
+    const lancirb200_plan_desc& d = pl->desc;
+    const size_t el = elem_size(d.in_type);
+    CUDA_TRY(cudaMemcpy2DAsync(seg, lhalo_row_bytes(d), static_cast<const char*>(band) + (size_t)r0 * src_pitch * el,
+                               src_pitch * el, (size_t)d.src_w * d.channels * el, n, cudaMemcpyDefault, st));
+    return 0;
+}
+
+// A band's passes: the column pass over its segmented source (s: the segments, flags and sequence number),
+// the row pass over its destination rows, full width.
+int lband(const lancirb200_plan* pl, const avirb200_shard_info& si, const void* band_src, size_t src_pitch,
+          void* band_dst, size_t dst_pitch, void* d_ws, LSeg s, cudaStream_t st) {
+    const lancirb200_plan_desc& d = pl->desc;
+    s.up0 = si.need_row0; s.row0 = si.src_row0; s.rows = si.src_rows;
+    // the edge rows: the leading and trailing destination rows whose clamped taps leave the band; the rows
+    // between must all stay inside it, or every row is an edge row (the tables need not be monotone)
+    const int kl = pl->dv.kl, n = si.dst_rows, r0 = si.src_row0, r1 = si.src_row0 + si.src_rows;
+    auto inside = [&](int y) {
+        const long long a = pl->pos_v[si.dst_row0 + y], b = a + kl - 1;
+        const long long ca = a < 0 ? 0 : (a >= d.src_h ? d.src_h - 1 : a), cb = b < 0 ? 0 : (b >= d.src_h ? d.src_h - 1 : b);
+        return ca >= r0 && cb < r1;
+    };
+    int top = 0, bot0 = n;
+    while (top < n && !inside(top)) ++top;
+    while (bot0 > top && !inside(bot0 - 1)) --bot0;
+    for (int y = top; y < bot0; ++y)
+        if (!inside(y)) {
+            top = bot0 = n;
+            break;
+        }
+    if (top >= bot0) top = bot0 = n;
+    s.top = top; s.bot0 = bot0;
+    return lancir_region(pl, 0, si.dst_row0, d.dst_w, si.dst_rows, 0, d.src_w, si.src_row0, band_src, src_pitch,
+                         band_dst, dst_pitch, d_ws, st, &s);
+}
+
+int lcheck(const lancirb200_plan* pl, size_t src_pitch, size_t dst_pitch) {
+    const lancirb200_plan_desc& d = pl->desc;
+    if (src_pitch < (size_t)d.src_w * d.channels || dst_pitch < (size_t)d.dst_w * d.channels)
+        return fail(AVIRB200_ERR_BAD_ARG, "pitch smaller than a row");
+    int cur = -1;
+    if (cudaGetDevice(&cur) != cudaSuccess || cur != pl->device)
+        return fail(AVIRB200_ERR_BAD_ARG, "the current device is not the plan's device");
+    return 0;
+}
+
+// lancirb200_resize_sharded for nranks > 1; the caller holds pl->mx.
+int lsharded(lancirb200_plan* pl, void* comm, int rank, int nranks, const void* d_src, size_t src_pitch, void* d_dst,
+             size_t dst_pitch, void* d_ws, cudaStream_t st) {
+    const lancirb200_plan_desc& d = pl->desc;
+    avirb200_shard_info si, up, dn; // this rank's bands and its neighbours'
+    std::memset(&up, 0, sizeof up);
+    std::memset(&dn, 0, sizeof dn);
+    int r = lshard_plan(pl, rank, nranks, &si);
+    if (r == 0 && rank > 0) r = lshard_plan(pl, rank - 1, nranks, &up);
+    if (r == 0 && rank + 1 < nranks) r = lshard_plan(pl, rank + 1, nranks, &dn);
+    if (r != 0) return r;
+    if (comm == nullptr) return fail(AVIRB200_ERR_BAD_ARG, "sharded resize needs a communicator");
+    avb::Nccl* nc = avb::nccl();
+    if (!nc) return fail(AVIRB200_ERR_NCCL, "libnccl.so.2 not loadable");
+    if (pl->opt_overlap && (!pl->halo || pl->halo->comm != comm || pl->halo->rank != rank || pl->halo->nranks != nranks)) {
+        if (pl->halo) {
+            avb::peer_boxes_close(pl->halo);
+            delete pl->halo;
+        }
+        LHalo* h = pl->halo = new LHalo(); // collective, once per plan
+        h->comm = comm; h->rank = rank; h->nranks = nranks;
+        h->mine = LBoxLayout(d, si);
+        h->above = LBoxLayout(d, up);
+        h->below = LBoxLayout(d, dn);
+        if ((r = avb::peer_boxes_open(comm, rank, nranks, h->mine.bytes(2), LBoxLayout::kHeader, st, h)) != 0) return r;
+    }
+    LHalo* h = (pl->opt_overlap && pl->halo && pl->halo->usable) ? pl->halo : nullptr;
+    // A pair of neighbours exchanges through the mailboxes when rows travel both ways (DESIGN.md section 7: then
+    // neither can run two calls ahead of the other); otherwise, and on the NCCL schedule, through NCCL.
+    const bool box_up = h && rank > 0 && si.halo_up > 0 && up.halo_down > 0;
+    const bool box_dn = h && rank + 1 < nranks && si.halo_down > 0 && dn.halo_up > 0;
+    const bool nccl_up = !box_up && rank > 0 && (si.halo_up > 0 || up.halo_down > 0);
+    const bool nccl_dn = !box_dn && rank + 1 < nranks && (si.halo_down > 0 || dn.halo_up > 0);
+    const LShardWs wl(d, si);
+    char* wsb = static_cast<char*>(d_ws);
+    const size_t el = elem_size(d.in_type), row16 = lhalo_row_bytes(d), rowb = (size_t)d.src_w * d.channels * el;
+    const char* srcb = static_cast<const char*>(d_src);
+    LSeg s;
+    std::memset(&s, 0, sizeof s);
+    s.up = wsb + wl.up; s.dn = wsb + wl.down;
+    s.up_pitch = s.dn_pitch = (long long)(row16 / el);
+    bool pushed = false;
+    if (box_up || box_dn) {
+        // the rows each neighbour needs go into its mailbox (this call's slot) on the exchange stream, each
+        // direction followed by the call's sequence number in the neighbour's flag; no kernel of this call
+        // comes before them
+        const unsigned seq = ++h->seq;
+        const int slot = (int)(seq & 1u);
+        unsigned* hs = &h->h_seq[seq & 63u];
+        *hs = seq;
+        s.seq = seq;
+        if ((r = lfork(pl, st)) != 0) return r;
+        if (box_up) {
+            if ((r = lcopy_rows(pl, h->above.from_down(h->box_up, slot), d_src, src_pitch, 0, up.halo_down, pl->stream_x)) != 0)
+                return r;
+            CUDA_TRY(cudaMemcpyAsync(h->box_up + 4, hs, 4, cudaMemcpyDefault, pl->stream_x));
+            s.up = h->mine.from_up(h->box, slot);
+            s.flag_up = reinterpret_cast<const volatile unsigned*>(h->box);
+        }
+        if (box_dn) {
+            if ((r = lcopy_rows(pl, h->below.from_up(h->box_down, slot), d_src, src_pitch, si.src_rows - dn.halo_up,
+                                dn.halo_up, pl->stream_x)) != 0)
+                return r;
+            CUDA_TRY(cudaMemcpyAsync(h->box_down, hs, 4, cudaMemcpyDefault, pl->stream_x));
+            s.dn = h->mine.from_down(h->box, slot);
+            s.flag_dn = reinterpret_cast<const volatile unsigned*>(h->box + 4);
+        }
+        CUDA_TRY(cudaEventRecord(pl->ev_x1, pl->stream_x));
+        pushed = true;
+    }
+    // the other pairs: one message per row into the workspace's halo segments, grouped before the column pass
+    if (nccl_up || nccl_dn) {
+        NCCL_TRY(nc->GroupStart());
+        if (nccl_up) {
+            for (int i = 0; i < up.halo_down; ++i)
+                NCCL_TRY(nc->Send(srcb + (size_t)i * src_pitch * el, rowb, 0, rank - 1, comm, st));
+            for (int i = 0; i < si.halo_up; ++i) NCCL_TRY(nc->Recv(wsb + wl.up + (size_t)i * row16, rowb, 0, rank - 1, comm, st));
+        }
+        if (nccl_dn) {
+            for (int i = si.src_rows - dn.halo_up; i < si.src_rows; ++i)
+                NCCL_TRY(nc->Send(srcb + (size_t)i * src_pitch * el, rowb, 0, rank + 1, comm, st));
+            for (int i = 0; i < si.halo_down; ++i)
+                NCCL_TRY(nc->Recv(wsb + wl.down + (size_t)i * row16, rowb, 0, rank + 1, comm, st));
+        }
+        NCCL_TRY(nc->GroupEnd());
+    }
+    r = lband(pl, si, d_src, src_pitch, d_dst, dst_pitch, d_ws, s, st);
+    // the pushes read the caller's source band: the caller's stream does not end before them
+    if (pushed) CUDA_TRY(cudaStreamWaitEvent(st, pl->ev_x1, 0));
+    return r;
+}
+
+} // namespace
+
+extern "C" {
+
+int lancirb200_plan_set_option(lancirb200_plan* pl, int option, int value) {
+    if (!pl) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
+    if (option != AVIRB200_OPT_OVERLAP_HALO) return fail(AVIRB200_ERR_BAD_ARG, "unknown option (CLancIR plans: AVIRB200_OPT_OVERLAP_HALO)");
+    if (value != 0 && value != 3) return fail(AVIRB200_ERR_BAD_ARG, "AVIRB200_OPT_OVERLAP_HALO: 3 (mailboxes) or 0 (NCCL)");
+    std::lock_guard<std::mutex> lk(pl->mx);
+    pl->opt_overlap = value;
+    return 0;
+}
+
+int lancirb200_shard_query(const lancirb200_plan* pl, int rank, int nranks, avirb200_shard_info* info) {
+    if (!pl || !info) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
+    return lshard_plan(pl, rank, nranks, info);
+}
+
+int lancirb200_shard_query_desc(const lancirb200_plan_desc* d, int rank, int nranks, avirb200_shard_info* info) {
+    if (!d || !info) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
+    if (d->src_w < 1 || d->src_h < 1 || d->dst_w < 1 || d->dst_h < 1 || !d->v.src_pos || d->v.dst_len < d->dst_h ||
+        d->v.kernel_len < 1)
+        return fail(AVIRB200_ERR_BAD_ARG, "bad geometry or axis tables");
+    return lshard(d->v.src_pos, d->v.kernel_len, d->src_h, d->dst_h, rank, nranks, info);
+}
+
+int lancirb200_shard_workspace_bytes(const lancirb200_plan* pl, int rank, int nranks, size_t* bytes) {
+    if (!pl || !bytes) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
+    avirb200_shard_info si;
+    const int r = lshard_plan(pl, rank, nranks, &si);
+    if (r != 0) return r;
+    *bytes = LShardWs(pl->desc, si).total;
+    return 0;
+}
+
+int lancirb200_resize_sharded(const lancirb200_plan* cpl, void* comm, int rank, int nranks, const void* d_src,
+                              size_t src_pitch, void* d_dst, size_t dst_pitch, void* d_ws, void* stream) {
+    if (!cpl || !d_src || !d_dst || !d_ws) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
+    avirb200_shard_info si;
+    int r = lshard_plan(cpl, rank, nranks, &si);
+    if (r == 0) r = lcheck(cpl, src_pitch, dst_pitch);
+    if (r != 0) return r;
+    if (nranks == 1) return lancirb200_resize_device(cpl, d_src, src_pitch, d_dst, dst_pitch, d_ws, stream);
+    lancirb200_plan* pl = const_cast<lancirb200_plan*>(cpl); // (exchange state is created on first use)
+    std::lock_guard<std::mutex> lk(pl->mx);
+    return lsharded(pl, comm, rank, nranks, d_src, src_pitch, d_dst, dst_pitch, d_ws, static_cast<cudaStream_t>(stream));
+}
+
+int lancirb200_resize_sharded_host(lancirb200_plan* pl, void* comm, int rank, int nranks, const void* h_src,
+                                   size_t src_pitch, void* h_dst, size_t dst_pitch) {
+    if (!pl || !h_src || !h_dst) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
+    const lancirb200_plan_desc& d = pl->desc;
+    avirb200_shard_info si;
+    int r = lshard_plan(pl, rank, nranks, &si);
+    if (r != 0) return r;
+    if (src_pitch < (size_t)d.src_w * d.channels || dst_pitch < (size_t)d.dst_w * d.channels)
+        return fail(AVIRB200_ERR_BAD_ARG, "pitch smaller than a row");
+    const size_t in_el = elem_size(d.in_type), out_el = elem_size(d.out_type);
+    const size_t in_row = (size_t)d.src_w * d.channels * in_el, out_row = (size_t)d.dst_w * d.channels * out_el;
+    std::lock_guard<std::mutex> lk(pl->mx);
+    // the call runs on the plan's device; the caller's current device is restored on every exit
+    struct DeviceGuard {
+        int prev = -1;
+        ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
+    } guard;
+    {
+        int cur = -1;
+        CUDA_TRY(cudaGetDevice(&cur));
+        if (cur != pl->device) {
+            CUDA_TRY(cudaSetDevice(pl->device));
+            guard.prev = cur;
+        }
+    }
+    if (!pl->stream) CUDA_TRY(cudaStreamCreateWithFlags(&pl->stream, cudaStreamNonBlocking));
+    if ((r = lgrow(&pl->d_src, &pl->src_bytes, in_row * si.src_rows)) != 0 ||
+        (r = lgrow(&pl->d_dst, &pl->dst_bytes, out_row * si.dst_rows)) != 0 ||
+        (r = lgrow(&pl->d_ws, &pl->ws_bytes, LShardWs(d, si).total)) != 0)
+        return r;
+    CUDA_TRY(cudaMemcpy2DAsync(pl->d_src, in_row, h_src, src_pitch * in_el, in_row, si.src_rows, cudaMemcpyHostToDevice,
+                               pl->stream));
+    const size_t sp = (size_t)d.src_w * d.channels, dp = (size_t)d.dst_w * d.channels;
+    r = nranks == 1 ? lancirb200_resize_device(pl, pl->d_src, sp, pl->d_dst, dp, pl->d_ws, pl->stream)
+                    : lsharded(pl, comm, rank, nranks, pl->d_src, sp, pl->d_dst, dp, pl->d_ws, pl->stream);
+    if (r != 0) return r;
+    CUDA_TRY(cudaMemcpy2DAsync(h_dst, dst_pitch * out_el, pl->d_dst, out_row, out_row, si.dst_rows, cudaMemcpyDeviceToHost,
+                               pl->stream));
+    CUDA_TRY(cudaStreamSynchronize(pl->stream));
+    return 0;
+}
+
+int lancirb200_resize_sharded_local(const lancirb200_plan* cpl, int nranks, const void* d_src, size_t src_pitch,
+                                    void* d_dst, size_t dst_pitch, void* d_ws, void* stream) {
+    if (!cpl || !d_src || !d_dst || !d_ws) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
+    if (nranks < 1) return fail(AVIRB200_ERR_BAD_ARG, "bad rank");
+    const lancirb200_plan_desc& d = cpl->desc;
+    std::vector<avirb200_shard_info> si(nranks);
+    std::vector<char*> ws(nranks);
+    std::vector<LShardWs> wl;
+    char* base = static_cast<char*>(d_ws);
+    for (int r = 0; r < nranks; ++r) { // every band's workspace: as lancirb200_shard_workspace_bytes lays it out
+        const int e = lshard_plan(cpl, r, nranks, &si[r]);
+        if (e != 0) return e;
+        wl.emplace_back(d, si[r]);
+        ws[r] = base;
+        base += wl[r].total;
+    }
+    int e = lcheck(cpl, src_pitch, dst_pitch);
+    if (e != 0) return e;
+    lancirb200_plan* pl = const_cast<lancirb200_plan*>(cpl); // (exchange state is created on first use)
+    std::lock_guard<std::mutex> lk(pl->mx);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const size_t in_el = elem_size(d.in_type), out_el = elem_size(d.out_type), el = in_el;
+    const char* srcb = static_cast<const char*>(d_src);
+    // The exchange of lancirb200_resize_sharded with every band's mailbox in its own workspace (the halo
+    // segments and the header's flags, one slot): the same push on the exchange stream and the same segmented
+    // column kernel waiting on the flags.  On the NCCL schedule (AVIRB200_OPT_OVERLAP_HALO = 0) the rows are
+    // copied into the same segments before the column passes, which then do not wait.
+    const bool box = pl->opt_overlap != 0 && nranks > 1;
+    cudaStream_t sx = st;
+    if (box) {
+        if (!pl->h_one) {
+            CUDA_TRY(cudaHostAlloc(&pl->h_one, sizeof(unsigned), cudaHostAllocPortable));
+            *pl->h_one = 1;
+        }
+        for (int r = 0; r < nranks; ++r) CUDA_TRY(cudaMemsetAsync(ws[r] + wl[r].header, 0, 8, st));
+        if ((e = lfork(pl, st)) != 0) return e;
+        sx = pl->stream_x;
+    }
+    for (int r = 0; r < nranks; ++r) {
+        const avirb200_shard_info& b = si[r];
+        if (b.halo_up > 0) { // band r-1's last rows
+            if ((e = lcopy_rows(pl, ws[r] + wl[r].up, srcb, src_pitch, b.need_row0, b.halo_up, sx)) != 0) return e;
+            if (box) CUDA_TRY(cudaMemcpyAsync(ws[r] + wl[r].header, pl->h_one, 4, cudaMemcpyDefault, sx));
+        }
+        if (b.halo_down > 0) { // band r+1's first rows
+            if ((e = lcopy_rows(pl, ws[r] + wl[r].down, srcb, src_pitch, b.src_row0 + b.src_rows, b.halo_down, sx)) != 0)
+                return e;
+            if (box) CUDA_TRY(cudaMemcpyAsync(ws[r] + wl[r].header + 4, pl->h_one, 4, cudaMemcpyDefault, sx));
+        }
+    }
+    if (box) CUDA_TRY(cudaEventRecord(pl->ev_x1, sx));
+    int r = 0;
+    for (int q = 0; q < nranks && r == 0; ++q) {
+        const avirb200_shard_info& b = si[q];
+        LSeg s;
+        std::memset(&s, 0, sizeof s);
+        s.up = ws[q] + wl[q].up; s.dn = ws[q] + wl[q].down;
+        s.up_pitch = s.dn_pitch = (long long)(lhalo_row_bytes(d) / el);
+        if (box) {
+            s.seq = 1;
+            if (b.halo_up > 0) s.flag_up = reinterpret_cast<const volatile unsigned*>(ws[q] + wl[q].header);
+            if (b.halo_down > 0) s.flag_dn = reinterpret_cast<const volatile unsigned*>(ws[q] + wl[q].header + 4);
+        }
+        r = lband(pl, b, srcb + (size_t)b.src_row0 * src_pitch * in_el, src_pitch,
+                  static_cast<char*>(d_dst) + (size_t)b.dst_row0 * dst_pitch * out_el, dst_pitch, ws[q], s, st);
+    }
+    if (box) CUDA_TRY(cudaStreamWaitEvent(st, pl->ev_x1, 0));
+    return r;
 }
 
 } // extern "C"

@@ -398,6 +398,50 @@ int lancirb200_resize_window_device(const lancirb200_plan* plan, int x0, int y0,
 int lancirb200_resize_window_host(lancirb200_plan* plan, int x0, int y0, int w, int h, const void* h_src,
                                   size_t src_pitch, void* h_dst, size_t dst_pitch);
 
+/* Row-sharded LANCIR (one process per GPU), as avirb200_*sharded* for AVIR: rank r of n holds source rows
+ * [src_h * r / n, src_h * (r + 1) / n) and produces destination rows [dst_h * r / n, dst_h * (r + 1) / n),
+ * bit-identical to the same rows of lancirb200_resize_device.  LANCIR resizes columns first, so only raw
+ * source rows travel between neighbours, in the caller's element type.  In avirb200_shard_info, need_row0 /
+ * need_rows are SOURCE rows: the band's vertical footprint (every tap position of its destination rows,
+ * clamped to the image, as lancirb200_window_query) joined with its own source band; halo_up / halo_down are
+ * the source rows of it held by rank-1 / rank+1.  AVIRB200_ERR_UNSUPPORTED, before any CUDA call, when a
+ * rank gets no rows, a halo is larger than the neighbour's band (too many ranks), or a band has more than
+ * 65535 destination rows (a plan taller than that runs sharded when every band fits). */
+int lancirb200_shard_query(const lancirb200_plan* plan, int rank, int nranks, avirb200_shard_info* info);
+/* Same, from a descriptor alone (no device needed). */
+int lancirb200_shard_query_desc(const lancirb200_plan_desc* desc, int rank, int nranks, avirb200_shard_info* info);
+/* The band's intermediate (dst_rows x src_w x channels floats), the two halo segments the NCCL schedule
+ * receives into and a 256-byte header. */
+int lancirb200_shard_workspace_bytes(const lancirb200_plan* plan, int rank, int nranks, size_t* bytes);
+/* d_src holds this rank's source band, d_dst receives its destination band; pitches in elements, at least a
+ * row.  `comm` is an ncclComm_t (avirb200_comm_create or the caller's own); nranks == 1 is
+ * lancirb200_resize_device.  The current device must be the plan's.  Asynchronous on `stream`; no allocation
+ * after the first call on a plan, which is collective (every rank makes it): every rank allocates a mailbox
+ * in device memory that its neighbours map through CUDA IPC (the handles travel over `comm`).  Per call a
+ * rank copies the rows each neighbour needs into that neighbour's mailbox on an exchange stream forked from
+ * `stream` (peer copies, no kernel of the call before them), then the call's sequence number into its flag;
+ * the column pass reads the neighbours' rows in place, and only its blocks whose taps reach them wait for
+ * the flag.  `stream` joins the exchange before the call returns.  A pair of neighbours where rows travel
+ * one way only, and every pair when some rank cannot map its neighbours or AVIRB200_OPT_OVERLAP_HALO is 0,
+ * exchanges with ncclSend / ncclRecv into the workspace's halo segments before the column pass. */
+int lancirb200_resize_sharded(const lancirb200_plan* plan, void* comm, int rank, int nranks, const void* d_src,
+                              size_t src_pitch, void* d_dst, size_t dst_pitch, void* d_workspace, void* stream);
+/* The same with HOST buffers (this rank's source band in, its destination band out), staged through the
+ * plan's buffers on the plan's stream, on the plan's device; synchronises; the caller's current device is
+ * unchanged afterwards. */
+int lancirb200_resize_sharded_host(lancirb200_plan* plan, void* comm, int rank, int nranks, const void* h_src,
+                                   size_t src_pitch, void* h_dst, size_t dst_pitch);
+/* Validation aid: every band of an `nranks` split on the CURRENT device, with full-image buffers.  The bands
+ * exchange through mailboxes in their own workspaces with the same push, segmented column kernel and flag
+ * protocol as ranks (AVIRB200_OPT_OVERLAP_HALO 0: device copies into the same segments, no waiting).
+ * d_workspace holds the sum of every rank's lancirb200_shard_workspace_bytes, band after band. */
+int lancirb200_resize_sharded_local(const lancirb200_plan* plan, int nranks, const void* d_src, size_t src_pitch,
+                                    void* d_dst, size_t dst_pitch, void* d_workspace, void* stream);
+/* CLancIR plans take one option, AVIRB200_OPT_OVERLAP_HALO: 3 (default, mailboxes) or 0 (every halo row
+ * through NCCL on lancirb200_resize_sharded, device copies on _local).  A test switch: results do not change
+ * by a bit.  Anything else is AVIRB200_ERR_BAD_ARG. */
+int lancirb200_plan_set_option(lancirb200_plan* plan, int option, int value);
+
 /* ---- misc ----------------------------------------------------------------------------- */
 
 const char* avirb200_status_string(int status);

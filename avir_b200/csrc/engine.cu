@@ -219,11 +219,11 @@ void build_dev_axis(HostAxis& ha, std::vector<char>& img, size_t& off, char* dba
     }
 }
 
+// grid.y: the blocks of lines, at most 65535 (the kernel loops over the rest).
 int launch_generic(const PassParams& p, const PassConfig& c, cudaStream_t st) {
-    dim3 grid((p.out1 - p.out0 + c.tile_out - 1) / c.tile_out,
-              (p.n_lines + c.lines_per_block - 1) / c.lines_per_block);
+    const int line_blocks = (p.n_lines + c.lines_per_block - 1) / c.lines_per_block;
+    dim3 grid((p.out1 - p.out0 + c.tile_out - 1) / c.tile_out, imin(line_blocks, 65535));
     if (grid.x == 0 || grid.y == 0) return 0;
-    if (grid.y > 65535) return fail(AVIRB200_ERR_UNSUPPORTED, "image too large for generic grid");
     if (p.sum_mode == AVIRB200_SUM_DIL8) {
         CUDA_TRY(raise_smem_limit(reinterpret_cast<const void*>(generic_pass_kernel<AVIRB200_SUM_DIL8>), c.smem));
         generic_pass_kernel<AVIRB200_SUM_DIL8><<<grid, 256, c.smem, st>>>(p);

@@ -200,19 +200,12 @@ __device__ float step_sample(const DevStep& s, const TileView& in, int j, int la
 
 // ---- the kernel -------------------------------------------------------------------------------
 
+// The tile of final outputs [j0, j1] of the lines [line0, line0 + nlines), every thread of the block.
 template <int SUM>
-__global__ void __launch_bounds__(256)
-generic_pass_kernel(const __grid_constant__ PassParams p) {
-    extern __shared__ float smem[];
-    float* bufs[2] = {smem, smem + (size_t)p.span_a * p.pitch};
-
+__device__ __forceinline__ void generic_tile(const PassParams& p, float* const bufs[2], int line0, int nlines,
+                                             int j0, int j1) {
     const int C = p.channels;
-    const int line0 = blockIdx.y * p.lines_per_block;
-    const int nlines = imin(p.lines_per_block, p.n_lines - line0);
     const int NL = nlines * C;
-    const int j0 = p.out0 + blockIdx.x * p.tile_out;
-    const int j1 = imin(j0 + p.tile_out, p.out1) - 1;
-    if (nlines <= 0 || j0 > j1) return;
 
     // Ranges every step must produce for this tile (uniform; a few integer ops).
     Range rng[AVIRB200_MAX_STEPS + 1];
@@ -287,6 +280,24 @@ generic_pass_kernel(const __grid_constant__ PassParams p) {
             const long long g = (long long)(line0 + r) * p.dst_pitch + (long long)(oa + pos - p.dst_row_base) * C + c;
             ((float*)p.dst)[g] = ob[pos * p.pitch + r * C + c];
         }
+    }
+}
+
+// blockIdx.x: a tile of outputs.  blockIdx.y: a block of lines, and every gridDim.y-th block after it: a pass
+// of more than 65535 line blocks (tall images, one line per block) runs in one launch of at most 65535 rows of
+// blocks.  Each output's arithmetic does not depend on which block computes it.
+template <int SUM>
+__global__ void __launch_bounds__(256)
+generic_pass_kernel(const __grid_constant__ PassParams p) {
+    extern __shared__ float smem[];
+    float* const bufs[2] = {smem, smem + (size_t)p.span_a * p.pitch};
+    const int j0 = p.out0 + blockIdx.x * p.tile_out;
+    const int j1 = imin(j0 + p.tile_out, p.out1) - 1;
+    if (j0 > j1) return;
+    for (long long line0 = (long long)blockIdx.y * p.lines_per_block; line0 < p.n_lines;
+         line0 += (long long)gridDim.y * p.lines_per_block) {
+        generic_tile<SUM>(p, bufs, (int)line0, imin(p.lines_per_block, p.n_lines - (int)line0), j0, j1);
+        __syncthreads(); // (the next block of lines stages its source over buffer 0)
     }
 }
 

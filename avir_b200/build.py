@@ -99,7 +99,7 @@ def _build_cuda(force=False, verbose=False):
     # chain and is compiled once per chain id (stream_types.h: StreamChainId 1..6) and pass, in parallel
     chains = list(range(1, 8))
     jobs = [(os.path.join(CSRC, n + ".cu"), os.path.join(PKG, n + ".o"), [])
-            for n in ("engine", "lancir", "peer_mailbox")]
+            for n in ("engine", "lancir", "peer_mailbox", "host_call")]
     jobs.append((os.path.join(CSRC, "stream_pass.cu"), os.path.join(PKG, "stream_pass.o"), []))
     jobs += [(os.path.join(CSRC, "stream_chain.cu"), os.path.join(PKG, "stream_chain_%d%s.o" % (k, "hv"[v])),
               ["-DAVS_CHAIN_ID=%d" % k, "-DAVS_CHAIN_PASS=%d" % v]) for k in chains for v in (0, 1)]

@@ -28,6 +28,7 @@
 #include "device_plan.h"
 #include "fast_pass.cuh"
 #include "generic_pass.cuh"
+#include "host_call.h"
 #include "host_util.h"
 #include "pass_config.h"
 #include "pass_request.h"
@@ -97,11 +98,8 @@ struct avirb200_plan {
     PassConfig cfg_h, cfg_v;
     FastPlan fast;
     avs::StreamAxisPlan stream_h, stream_v; // chain != 0: the pass runs on the streaming kernel
-    // resize_host: the device's shared staging buffers for the duration of a call
+    // held by host calls (host_call.h) and by sharded calls of more than one rank; host calls run on `stream`
     std::mutex mx;
-    void* d_src = nullptr;
-    void* d_dst = nullptr;
-    void* d_ws = nullptr;
     cudaStream_t stream = nullptr;
     // pipelined resize_host: copy-in / copy-out streams and per-band events
     cudaStream_t stream_in = nullptr, stream_out = nullptr;
@@ -784,17 +782,7 @@ int finish_rows(const avirb200_plan* pl, const float* out32, float* bnd, int* pr
     return 0;
 }
 
-// ---- host-call staging: one set of device buffers per device, shared by every plan ----------------
-// (a front-end object caches up to 16 plans; per-plan staging of 8K frames would hold ~1 GB each)
-struct Staging {
-    std::mutex mx; // held for the whole host call: host calls on one device run one at a time
-    void *d_src = nullptr, *d_dst = nullptr, *d_ws = nullptr;
-    size_t src_b = 0, dst_b = 0, ws_b = 0;
-    // page-locked bounce buffers for callers' pageable (malloc) images: a ring of source bands
-    // and the whole destination
-    char *h_in = nullptr, *h_out = nullptr;
-    size_t h_in_b = 0, h_out_b = 0;
-};
+// ---- banded host calls: pageable images through page-locked bounce buffers ------------------------
 
 // A few host threads that move image rows between the caller's pageable memory and the
 // page-locked bounce buffers (one thread's memcpy is slower than PCIe).
@@ -876,29 +864,6 @@ int grow_host(char** p, size_t* have, size_t need) {
     *p = nullptr; *have = 0;
     CUDA_TRY(cudaHostAlloc(reinterpret_cast<void**>(p), need, cudaHostAllocDefault));
     *have = need;
-    return 0;
-}
-Staging& staging_of(int device) {
-    static Staging pool[64];
-    return pool[(unsigned)device & 63u];
-}
-int grow(void** p, size_t* have, size_t need) {
-    if (*have >= need) return 0;
-    cudaFree(*p);
-    *p = nullptr; *have = 0;
-    CUDA_TRY(cudaMalloc(p, need));
-    *have = need;
-    return 0;
-}
-// Points the plan's d_src / d_dst / d_ws at the device's staging buffers (grown to the sizes
-// asked for).  The caller holds staging_of(pl->device).mx.
-int plan_staging(avirb200_plan* pl, size_t in_bytes, size_t out_bytes, size_t ws) {
-    Staging& sg = staging_of(pl->device);
-    int r;
-    if ((r = grow(&sg.d_src, &sg.src_b, in_bytes)) != 0 || (r = grow(&sg.d_dst, &sg.dst_b, out_bytes)) != 0 ||
-        (r = grow(&sg.d_ws, &sg.ws_b, ws)) != 0)
-        return r;
-    pl->d_src = sg.d_src; pl->d_dst = sg.d_dst; pl->d_ws = sg.d_ws;
     return 0;
 }
 
@@ -1414,43 +1379,21 @@ int avirb200_resize_window_host(avirb200_plan* pl, int x0, int y0, int w, int h,
                                 size_t src_pitch, void* h_dst, size_t dst_pitch) {
     if (pl == nullptr || h_src == nullptr || h_dst == nullptr) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
     const avirb200_plan_desc& d = pl->desc;
-    if (src_pitch < (size_t)d.src_w * d.channels || dst_pitch < (size_t)w * d.channels)
-        return fail(AVIRB200_ERR_BAD_ARG, "pitch smaller than a row");
     avirb200_window_info wi;
-    int r = window_compute(pl->h.hostdev, pl->v.hostdev, pl->errd, x0, y0, w, h, &wi);
+    const int r = window_compute(pl->h.hostdev, pl->v.hostdev, pl->errd, x0, y0, w, h, &wi);
     if (r != 0) return r;
-    std::lock_guard<std::mutex> lk(pl->mx);
-    // the call runs on the plan's device; the caller's current device is restored on every exit
-    struct DeviceGuard {
-        int prev = -1;
-        ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
-    } guard;
-    {
-        int cur = -1;
-        CUDA_TRY(cudaGetDevice(&cur));
-        if (cur != pl->device) {
-            CUDA_TRY(cudaSetDevice(pl->device));
-            guard.prev = cur;
-        }
-    }
-    size_t ws = 0;
-    if ((r = avirb200_window_workspace_bytes(pl, x0, y0, w, h, &ws)) != 0) return r;
-    std::lock_guard<std::mutex> sl(staging_of(pl->device).mx);
-    const size_t in_el = elem_size(pl->io_in_type), out_el = elem_size(pl->io_out_type);
-    const size_t in_row = (size_t)wi.src_w * d.channels * in_el, out_row = (size_t)w * d.channels * out_el;
-    if (pl->stream == nullptr) CUDA_TRY(cudaStreamCreateWithFlags(&pl->stream, cudaStreamNonBlocking));
-    if ((r = plan_staging(pl, in_row * wi.src_h, out_row * h, ws)) != 0) return r;
     // the footprint only; the whole source is read before any destination pixel is written (aliasing)
-    const char* fsrc = static_cast<const char*>(h_src) + ((size_t)wi.src_y0 * src_pitch + (size_t)wi.src_x0 * d.channels) * in_el;
-    CUDA_TRY(cudaMemcpy2DAsync(pl->d_src, in_row, fsrc, src_pitch * in_el, in_row, wi.src_h, cudaMemcpyHostToDevice,
-                               pl->stream));
-    r = resize_region(pl, &wi, x0, y0, w, h, pl->d_src, (size_t)wi.src_w * d.channels, pl->d_dst, (size_t)w * d.channels,
-                      pl->d_ws, pl->stream);
-    if (r != 0) return r;
-    CUDA_TRY(cudaMemcpy2DAsync(h_dst, dst_pitch * out_el, pl->d_dst, out_row, out_row, h, cudaMemcpyDeviceToHost,
-                               pl->stream));
-    CUDA_TRY(cudaStreamSynchronize(pl->stream));
-    return 0;
+    const size_t C = d.channels;
+    const HostRect src = host_rect(h_src, src_pitch, d.src_w * C, elem_size(pl->io_in_type), wi.src_x0 * C, wi.src_w * C,
+                                   wi.src_y0, wi.src_h);
+    const HostRect dst = host_rect(h_dst, dst_pitch, w * C, elem_size(pl->io_out_type), 0, w * C, 0, h);
+    return staged_call(pl->mx, staging_of(pl->device), pl->device, &pl->stream, src, dst, ws_layout(pl, wi, w, h).total,
+                       [&](const void* s, void* o, void* ws, cudaStream_t st) {
+                           // (the tile kernel's tables of the window's ranges, on the plan's device)
+                           fast_prepare_columns(pl->fast, x0, x0 + w);
+                           fast_prepare_range(pl->fast, y0, y0 + h);
+                           return resize_region(pl, &wi, x0, y0, w, h, s, wi.src_w * C, o, w * C, ws, st);
+                       });
 }
 
 int avirb200_row_pass_device(const avirb200_plan* pl, const void* d_src, size_t src_pitch,
@@ -1521,32 +1464,12 @@ int avirb200_resize_host(avirb200_plan* pl, const void* h_src, size_t src_pitch,
     if (pl == nullptr || h_src == nullptr || h_dst == nullptr)
         return fail(AVIRB200_ERR_BAD_ARG, "null argument");
     const avirb200_plan_desc& d = pl->desc;
-    std::lock_guard<std::mutex> lk(pl->mx);
-    // the call runs on the plan's device; the caller's current device is restored on every exit
-    struct DeviceGuard {
-        int prev = -1;
-        ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
-    } guard;
-    {
-        int cur = -1;
-        CUDA_TRY(cudaGetDevice(&cur));
-        if (cur != pl->device) {
-            CUDA_TRY(cudaSetDevice(pl->device));
-            guard.prev = cur;
-        }
-    }
-    std::lock_guard<std::mutex> sl(staging_of(pl->device).mx);
-    const size_t in_row = (size_t)d.src_w * d.channels * elem_size(pl->io_in_type);
-    const size_t out_row = (size_t)d.dst_w * d.channels * elem_size(pl->io_out_type);
-    const size_t in_bytes = in_row * d.src_h, out_bytes = out_row * d.dst_h;
-    size_t ws = 0;
-    avirb200_plan_workspace_bytes(pl, &ws);
-    if (pl->stream == nullptr) CUDA_TRY(cudaStreamCreateWithFlags(&pl->stream, cudaStreamNonBlocking));
-    {
-        const int r0 = plan_staging(pl, in_bytes, out_bytes, ws);
-        if (r0 != 0) return r0;
-    }
     const size_t in_el = elem_size(pl->io_in_type), out_el = elem_size(pl->io_out_type);
+    const size_t sw = (size_t)d.src_w * d.channels, dw = (size_t)d.dst_w * d.channels;
+    const HostRect src = host_rect(h_src, src_pitch, sw, in_el, 0, sw, 0, d.src_h);
+    const HostRect dst = host_rect(h_dst, dst_pitch, dw, out_el, 0, dw, 0, d.dst_h);
+    const size_t in_row = src.row, out_row = dst.row;
+    const size_t in_bytes = in_row * d.src_h, out_bytes = out_row * d.dst_h;
     // Pipelined form for large images: the image is cut into row bands (the multi-GPU band
     // arithmetic, one shared intermediate buffer instead of a halo exchange).  Band b's rows
     // travel host->device on the copy-in stream while the kernels of band b-1 run on the
@@ -1574,6 +1497,12 @@ int avirb200_resize_host(avirb200_plan* pl, const void* h_src, size_t src_pitch,
         nb /= 2;
     }
     if (nb >= 2) {
+        HostCall call(pl->mx, staging_of(pl->device));
+        {
+            const int r0 = call.begin(pl->device, &pl->stream, src, dst, ws_layout(pl).total);
+            if (r0 != 0) return r0;
+        }
+        Staging& sg = call.sg;
         // the tile kernel's tables of the bands' destination rows (a launch does not build them)
         for (int b = 0; b < nb; ++b) fast_prepare_range(pl->fast, si[b].dst_row0, si[b].dst_row0 + si[b].dst_rows);
         if (pl->stream_in == nullptr) CUDA_TRY(cudaStreamCreateWithFlags(&pl->stream_in, cudaStreamNonBlocking));
@@ -1586,9 +1515,8 @@ int avirb200_resize_host(avirb200_plan* pl, const void* h_src, size_t src_pitch,
             pl->ev_out.push_back(e1);
         }
         const size_t rowf = mid_pitch(pl);
-        const size_t dsrc_pitch = (size_t)d.src_w * d.channels, ddst_pitch = (size_t)d.dst_w * d.channels;
-        char* src4 = static_cast<char*>(pl->d_ws) + ws_layout(pl).src4;
-        char* dst4 = static_cast<char*>(pl->d_ws) + ws_layout(pl).dst4;
+        char* src4 = static_cast<char*>(sg.d_ws) + ws_layout(pl).src4;
+        char* dst4 = static_cast<char*>(sg.d_ws) + ws_layout(pl).dst4;
         const size_t src4_row = (size_t)d.src_w * 4 * in_el, dst4_row = (size_t)d.dst_w * 4 * out_el;
         int launches = 0;
         // Pageable (malloc) caller buffers: a copy call straight from / to them returns only when
@@ -1599,7 +1527,6 @@ int avirb200_resize_host(avirb200_plan* pl, const void* h_src, size_t src_pitch,
         // whole-image buffer drained band by band by a helper thread.
         constexpr int kInSlots = 3;
         const bool stage_in = is_pageable(h_src), stage_out = is_pageable(h_dst);
-        Staging& sg = staging_of(pl->device);
         size_t slot_bytes = 0;
         for (int b = 0; b < nb; ++b) slot_bytes = std::max(slot_bytes, align_up((size_t)si[b].src_rows * in_row, 4096));
         if (stage_in) { const int r0 = grow_host(&sg.h_in, &sg.h_in_b, slot_bytes * kInSlots); if (r0 != 0) return r0; }
@@ -1638,13 +1565,13 @@ int avirb200_resize_host(avirb200_plan* pl, const void* h_src, size_t src_pitch,
                 char* hs = sg.h_in + (size_t)slot * slot_bytes;
                 CopyPool::get().copy2d(hs, in_row, static_cast<const char*>(h_src) + (size_t)si[b].src_row0 * src_pitch * in_el,
                                        src_pitch * in_el, in_row, si[b].src_rows);
-                CUDA_TRY(cudaMemcpyAsync(static_cast<char*>(pl->d_src) + (size_t)si[b].src_row0 * in_row, hs,
+                CUDA_TRY(cudaMemcpyAsync(static_cast<char*>(sg.d_src) + (size_t)si[b].src_row0 * in_row, hs,
                                          (size_t)si[b].src_rows * in_row, cudaMemcpyHostToDevice, pl->stream_in));
                 CUDA_TRY(cudaEventRecord(pl->ev_slot[slot], pl->stream_in));
                 CUDA_TRY(cudaEventRecord(pl->ev_in[b], pl->stream_in));
                 return 0;
             }
-            CUDA_TRY(cudaMemcpy2DAsync(static_cast<char*>(pl->d_src) + (size_t)si[b].src_row0 * in_row, in_row,
+            CUDA_TRY(cudaMemcpy2DAsync(static_cast<char*>(sg.d_src) + (size_t)si[b].src_row0 * in_row, in_row,
                                        static_cast<const char*>(h_src) + (size_t)si[b].src_row0 * src_pitch * in_el,
                                        src_pitch * in_el, in_row, si[b].src_rows, cudaMemcpyHostToDevice,
                                        pl->stream_in));
@@ -1653,8 +1580,8 @@ int avirb200_resize_host(avirb200_plan* pl, const void* h_src, size_t src_pitch,
         };
         { const int r0 = copy_in(0); if (r0 != 0) return r0; }
         auto col_band = [&](int b) -> int {
-            char* dd = static_cast<char*>(pl->d_dst) + (size_t)si[b].dst_row0 * out_row;
-            PassRequest q = col_request(d, d.dst_w, static_cast<const float*>(pl->d_ws), rowf, 0, d.src_h, dd, ddst_pitch,
+            char* dd = static_cast<char*>(sg.d_dst) + (size_t)si[b].dst_row0 * out_row;
+            PassRequest q = col_request(d, d.dst_w, static_cast<const float*>(sg.d_ws), rowf, 0, d.src_h, dd, dw,
                                         si[b].dst_row0, si[b].dst_row0 + si[b].dst_rows);
             q.scratch4 = dst4 + (size_t)si[b].dst_row0 * dst4_row;
             const int r = run_pass(pl, q, pl->stream, &launches);
@@ -1676,8 +1603,8 @@ int avirb200_resize_host(avirb200_plan* pl, const void* h_src, size_t src_pitch,
         for (int b = 0; b < nb; ++b) {
             if (b + 1 < nb) { const int r0 = copy_in(b + 1); if (r0 != 0) return r0; }
             CUDA_TRY(cudaStreamWaitEvent(pl->stream, pl->ev_in[b], 0));
-            PassRequest q = row_request(d, static_cast<const char*>(pl->d_src) + (size_t)si[b].src_row0 * in_row, dsrc_pitch,
-                                        si[b].src_rows, static_cast<float*>(pl->d_ws) + (size_t)si[b].src_row0 * rowf, rowf);
+            PassRequest q = row_request(d, static_cast<const char*>(sg.d_src) + (size_t)si[b].src_row0 * in_row, sw,
+                                        si[b].src_rows, static_cast<float*>(sg.d_ws) + (size_t)si[b].src_row0 * rowf, rowf);
             q.scratch4 = src4 + (size_t)si[b].src_row0 * src4_row;
             int r = run_pass(pl, q, pl->stream, &launches);
             if (r != 0) return r;
@@ -1691,15 +1618,10 @@ int avirb200_resize_host(avirb200_plan* pl, const void* h_src, size_t src_pitch,
         if (drainer.t.joinable()) drainer.t.join(); // the last bands reach the caller's memory
         return 0;
     }
-    CUDA_TRY(cudaMemcpy2DAsync(pl->d_src, in_row, h_src, src_pitch * in_el, in_row,
-                               d.src_h, cudaMemcpyHostToDevice, pl->stream));
-    int r = avirb200_resize_device(pl, pl->d_src, (size_t)d.src_w * d.channels, pl->d_dst,
-                                   (size_t)d.dst_w * d.channels, pl->d_ws, pl->stream);
-    if (r != 0) return r;
-    CUDA_TRY(cudaMemcpy2DAsync(h_dst, dst_pitch * out_el, pl->d_dst, out_row,
-                               out_row, d.dst_h, cudaMemcpyDeviceToHost, pl->stream));
-    CUDA_TRY(cudaStreamSynchronize(pl->stream));
-    return 0;
+    return staged_call(pl->mx, staging_of(pl->device), pl->device, &pl->stream, src, dst, ws_layout(pl).total,
+                       [&](const void* s, void* o, void* ws, cudaStream_t st) {
+                           return avirb200_resize_device(pl, s, sw, o, dw, ws, st);
+                       });
 }
 
 // ---- sharded ---------------------------------------------------------------------------------
@@ -1765,18 +1687,18 @@ void avirb200_comm_destroy(void* comm) {
     if (nc && nc->CommDestroy && comm) nc->CommDestroy(comm);
 }
 
-int avirb200_resize_sharded(const avirb200_plan* cpl, void* comm, int rank, int nranks,
-                            const void* d_src, size_t src_pitch, void* d_dst, size_t dst_pitch,
-                            void* d_ws, void* stream) {
-    if (cpl == nullptr || d_src == nullptr || d_dst == nullptr || d_ws == nullptr)
-        return fail(AVIRB200_ERR_BAD_ARG, "null argument");
-    avirb200_plan* pl = const_cast<avirb200_plan*>(cpl); // (exchange state is created on first use)
+} // extern "C"
+
+namespace {
+
+// avirb200_resize_sharded; for nranks > 1 the caller holds pl->mx.
+int sharded(avirb200_plan* pl, void* comm, int rank, int nranks, const void* d_src, size_t src_pitch, void* d_dst,
+            size_t dst_pitch, void* d_ws, cudaStream_t st) {
     { int cur = -1; if (cudaGetDevice(&cur) != cudaSuccess || cur != pl->device) return fail(AVIRB200_ERR_BAD_ARG, "the current device is not the plan's device"); }
     avirb200_shard_info si;
     int r = shard_compute(pl, rank, nranks, &si);
     if (r != 0) return r;
     const avirb200_plan_desc& d = pl->desc;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
     const size_t rowf = mid_pitch(pl);
     const size_t in_el = elem_size(d.in_type);
     float* mid = static_cast<float*>(d_ws);
@@ -1831,7 +1753,6 @@ int avirb200_resize_sharded(const avirb200_plan* cpl, void* comm, int rank, int 
     link.dn = (rank + 1 < nranks) ? &down : nullptr;
     const int top_rows = avs::stream_rows_up(link), bot_rows = avs::stream_rows_down(link);
 
-    std::lock_guard<std::mutex> lk(pl->mx);
     if (pl->opt_overlap) {
         if (pl->halo == nullptr || pl->halo->comm != comm || pl->halo->rank != rank || pl->halo->nranks != nranks) {
             r = halo_setup(pl, comm, rank, nranks, st); // collective, once per plan
@@ -1985,38 +1906,39 @@ int avirb200_resize_sharded(const avirb200_plan* cpl, void* comm, int rank, int 
     return r;
 }
 
+} // namespace
+
+extern "C" {
+
+int avirb200_resize_sharded(const avirb200_plan* cpl, void* comm, int rank, int nranks,
+                            const void* d_src, size_t src_pitch, void* d_dst, size_t dst_pitch,
+                            void* d_ws, void* stream) {
+    if (cpl == nullptr || d_src == nullptr || d_dst == nullptr || d_ws == nullptr)
+        return fail(AVIRB200_ERR_BAD_ARG, "null argument");
+    avirb200_plan* pl = const_cast<avirb200_plan*>(cpl); // (exchange state is created on first use)
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (nranks <= 1) return sharded(pl, comm, rank, nranks, d_src, src_pitch, d_dst, dst_pitch, d_ws, st);
+    std::lock_guard<std::mutex> lk(pl->mx);
+    return sharded(pl, comm, rank, nranks, d_src, src_pitch, d_dst, dst_pitch, d_ws, st);
+}
+
 int avirb200_resize_sharded_host(avirb200_plan* pl, void* comm, int rank, int nranks, const void* h_src,
                                  size_t src_pitch, void* h_dst, size_t dst_pitch) {
     if (pl == nullptr || h_src == nullptr || h_dst == nullptr) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
     const avirb200_plan_desc& d = pl->desc;
     avirb200_shard_info si;
-    int r = shard_compute(pl, rank, nranks, &si);
+    const int r = shard_compute(pl, rank, nranks, &si);
     if (r != 0) return r;
-    size_t ws = 0;
-    if ((r = avirb200_shard_workspace_bytes(pl, rank, nranks, &ws)) != 0) return r;
     // (the caller's element types: double bands are staged as doubles, dithered ones as integers)
-    const size_t in_el = elem_size(pl->io_in_type), out_el = elem_size(pl->io_out_type);
-    const size_t in_row = (size_t)d.src_w * d.channels * in_el;
-    const size_t out_row = (size_t)d.dst_w * d.channels * out_el;
-    {
-        std::lock_guard<std::mutex> lk(pl->mx);
-        int cur = -1;
-        if (cudaGetDevice(&cur) != cudaSuccess || cur != pl->device)
-            return fail(AVIRB200_ERR_BAD_ARG, "the current device is not the plan's device");
-        if (pl->stream == nullptr) CUDA_TRY(cudaStreamCreateWithFlags(&pl->stream, cudaStreamNonBlocking));
-    }
-    std::lock_guard<std::mutex> sl(staging_of(pl->device).mx);
-    r = plan_staging(pl, in_row * si.src_rows, out_row * si.dst_rows, ws);
-    if (r != 0) return r;
-    CUDA_TRY(cudaMemcpy2DAsync(pl->d_src, in_row, h_src, src_pitch * in_el, in_row, si.src_rows,
-                               cudaMemcpyHostToDevice, pl->stream));
-    r = avirb200_resize_sharded(pl, comm, rank, nranks, pl->d_src, (size_t)d.src_w * d.channels, pl->d_dst,
-                                (size_t)d.dst_w * d.channels, pl->d_ws, pl->stream);
-    if (r != 0) return r;
-    CUDA_TRY(cudaMemcpy2DAsync(h_dst, dst_pitch * out_el, pl->d_dst, out_row, out_row, si.dst_rows,
-                               cudaMemcpyDeviceToHost, pl->stream));
-    CUDA_TRY(cudaStreamSynchronize(pl->stream));
-    return 0;
+    const size_t sw = (size_t)d.src_w * d.channels, dw = (size_t)d.dst_w * d.channels;
+    const HostRect src = host_rect(h_src, src_pitch, sw, elem_size(pl->io_in_type), 0, sw, 0, si.src_rows);
+    const HostRect dst = host_rect(h_dst, dst_pitch, dw, elem_size(pl->io_out_type), 0, dw, 0, si.dst_rows);
+    return staged_call(pl->mx, staging_of(pl->device), pl->device, &pl->stream, src, dst, ws_layout(pl, si).total,
+                       [&](const void* s, void* o, void* ws, cudaStream_t st) {
+                           // (the tile kernel's table of the band's rows, on the plan's device)
+                           fast_prepare_range(pl->fast, si.dst_row0, si.dst_row0 + si.dst_rows);
+                           return sharded(pl, comm, rank, nranks, s, sw, o, dw, ws, st);
+                       });
 }
 
 int avirb200_resize_sharded_local(const avirb200_plan* pl, int nranks, const void* d_src,

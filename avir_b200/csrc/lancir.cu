@@ -39,6 +39,7 @@
 #include <vector>
 
 #include "avirb200.h"
+#include "host_call.h"
 #include "host_util.h"
 #include "peer_mailbox.h"
 
@@ -556,10 +557,7 @@ struct lancirb200_plan {
     std::vector<int32_t> pos_v, pos_h; // host copies of the axes' src_pos (window footprints)
     int device = 0;
     std::mutex mx;
-    void* d_src = nullptr;
-    void* d_dst = nullptr;
-    void* d_ws = nullptr;
-    size_t src_bytes = 0, dst_bytes = 0, ws_bytes = 0;
+    avb::Staging staging;        // host calls: this plan's own staging buffers (host_call.h)
     cudaStream_t stream = nullptr;
     // row-sharded calls
     int opt_overlap = 3;           // AVIRB200_OPT_OVERLAP_HALO: 3 mailboxes, 0 NCCL
@@ -633,7 +631,7 @@ int lancirb200_plan_create(const lancirb200_plan_desc* d, lancirb200_plan** out)
 
 void lancirb200_plan_destroy(lancirb200_plan* pl) {
     if (!pl) return;
-    cudaFree(pl->arena); cudaFree(pl->d_src); cudaFree(pl->d_dst); cudaFree(pl->d_ws);
+    cudaFree(pl->arena);
     if (pl->stream) cudaStreamDestroy(pl->stream);
     if (pl->halo) {
         avb::peer_boxes_close(pl->halo);
@@ -772,46 +770,15 @@ int lancirb200_resize_host(lancirb200_plan* pl, const void* h_src, size_t src_pi
                            size_t dst_pitch) {
     if (!pl || !h_src || !h_dst) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
     const lancirb200_plan_desc& d = pl->desc;
-    std::lock_guard<std::mutex> lk(pl->mx);
-    // the call runs on the plan's device; the caller's current device is restored on every exit
-    struct DeviceGuard {
-        int prev = -1;
-        ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
-    } guard;
-    {
-        int cur = -1;
-        CUDA_TRY(cudaGetDevice(&cur));
-        if (cur != pl->device) {
-            CUDA_TRY(cudaSetDevice(pl->device));
-            guard.prev = cur;
-        }
-    }
-    const size_t in_row = (size_t)d.src_w * d.channels * elem_size(d.in_type);
-    const size_t out_row = (size_t)d.dst_w * d.channels * elem_size(d.out_type);
+    const size_t sw = (size_t)d.src_w * d.channels, dw = (size_t)d.dst_w * d.channels;
+    const avb::HostRect src = avb::host_rect(h_src, src_pitch, sw, elem_size(d.in_type), 0, sw, 0, d.src_h);
+    const avb::HostRect dst = avb::host_rect(h_dst, dst_pitch, dw, elem_size(d.out_type), 0, dw, 0, d.dst_h);
     size_t ws = 0;
     lancirb200_plan_workspace_bytes(pl, &ws);
-    if (!pl->stream) CUDA_TRY(cudaStreamCreateWithFlags(&pl->stream, cudaStreamNonBlocking));
-    if (pl->src_bytes < in_row * d.src_h) {
-        cudaFree(pl->d_src); pl->d_src = nullptr; pl->src_bytes = 0;
-        CUDA_TRY(cudaMalloc(&pl->d_src, in_row * d.src_h)); pl->src_bytes = in_row * d.src_h;
-    }
-    if (pl->dst_bytes < out_row * d.dst_h) {
-        cudaFree(pl->d_dst); pl->d_dst = nullptr; pl->dst_bytes = 0;
-        CUDA_TRY(cudaMalloc(&pl->d_dst, out_row * d.dst_h)); pl->dst_bytes = out_row * d.dst_h;
-    }
-    if (pl->ws_bytes < ws) {
-        cudaFree(pl->d_ws); pl->d_ws = nullptr; pl->ws_bytes = 0;
-        CUDA_TRY(cudaMalloc(&pl->d_ws, ws)); pl->ws_bytes = ws;
-    }
-    CUDA_TRY(cudaMemcpy2DAsync(pl->d_src, in_row, h_src, src_pitch * elem_size(d.in_type), in_row,
-                                d.src_h, cudaMemcpyHostToDevice, pl->stream));
-    int r = lancirb200_resize_device(pl, pl->d_src, (size_t)d.src_w * d.channels, pl->d_dst,
-                                     (size_t)d.dst_w * d.channels, pl->d_ws, pl->stream);
-    if (r != 0) return r;
-    CUDA_TRY(cudaMemcpy2DAsync(h_dst, dst_pitch * elem_size(d.out_type), pl->d_dst, out_row, out_row,
-                                d.dst_h, cudaMemcpyDeviceToHost, pl->stream));
-    CUDA_TRY(cudaStreamSynchronize(pl->stream));
-    return 0;
+    return avb::staged_call(pl->mx, pl->staging, pl->device, &pl->stream, src, dst, ws,
+                            [&](const void* s, void* o, void* w, cudaStream_t st) {
+                                return lancirb200_resize_device(pl, s, sw, o, dw, w, st);
+                            });
 }
 
 int lancirb200_window_query(const lancirb200_plan* pl, int x0, int y0, int w, int h, lancirb200_window_info* info) {
@@ -856,51 +823,19 @@ int lancirb200_resize_window_host(lancirb200_plan* pl, int x0, int y0, int w, in
     if (!pl || !h_src || !h_dst) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
     const lancirb200_plan_desc& d = pl->desc;
     lancirb200_window_info wi;
-    int r = lancir_window(pl, x0, y0, w, h, &wi);
+    const int r = lancir_window(pl, x0, y0, w, h, &wi);
     if (r != 0) return r;
-    if (src_pitch < (size_t)d.src_w * d.channels || dst_pitch < (size_t)w * d.channels)
-        return fail(AVIRB200_ERR_BAD_ARG, "pitch smaller than a row");
-    std::lock_guard<std::mutex> lk(pl->mx);
-    // the call runs on the plan's device; the caller's current device is restored on every exit
-    struct DeviceGuard {
-        int prev = -1;
-        ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
-    } guard;
-    {
-        int cur = -1;
-        CUDA_TRY(cudaGetDevice(&cur));
-        if (cur != pl->device) {
-            CUDA_TRY(cudaSetDevice(pl->device));
-            guard.prev = cur;
-        }
-    }
-    const size_t in_el = elem_size(d.in_type), out_el = elem_size(d.out_type);
-    const size_t in_row = (size_t)wi.src_w * d.channels * in_el, out_row = (size_t)w * d.channels * out_el;
-    const size_t ws = (size_t)h * wi.src_w * d.channels * sizeof(float);
-    if (!pl->stream) CUDA_TRY(cudaStreamCreateWithFlags(&pl->stream, cudaStreamNonBlocking));
-    if (pl->src_bytes < in_row * wi.src_h) {
-        cudaFree(pl->d_src); pl->d_src = nullptr; pl->src_bytes = 0;
-        CUDA_TRY(cudaMalloc(&pl->d_src, in_row * wi.src_h)); pl->src_bytes = in_row * wi.src_h;
-    }
-    if (pl->dst_bytes < out_row * h) {
-        cudaFree(pl->d_dst); pl->d_dst = nullptr; pl->dst_bytes = 0;
-        CUDA_TRY(cudaMalloc(&pl->d_dst, out_row * h)); pl->dst_bytes = out_row * h;
-    }
-    if (pl->ws_bytes < ws) {
-        cudaFree(pl->d_ws); pl->d_ws = nullptr; pl->ws_bytes = 0;
-        CUDA_TRY(cudaMalloc(&pl->d_ws, ws)); pl->ws_bytes = ws;
-    }
     // the footprint only
-    const char* fsrc = static_cast<const char*>(h_src) + ((size_t)wi.src_y0 * src_pitch + (size_t)wi.src_x0 * d.channels) * in_el;
-    CUDA_TRY(cudaMemcpy2DAsync(pl->d_src, in_row, fsrc, src_pitch * in_el, in_row, wi.src_h, cudaMemcpyHostToDevice,
-                               pl->stream));
-    r = lancir_region(pl, x0, y0, w, h, wi.src_x0, wi.src_w, wi.src_y0, pl->d_src, (size_t)wi.src_w * d.channels,
-                      pl->d_dst, (size_t)w * d.channels, pl->d_ws, pl->stream);
-    if (r != 0) return r;
-    CUDA_TRY(cudaMemcpy2DAsync(h_dst, dst_pitch * out_el, pl->d_dst, out_row, out_row, h, cudaMemcpyDeviceToHost,
-                               pl->stream));
-    CUDA_TRY(cudaStreamSynchronize(pl->stream));
-    return 0;
+    const size_t C = d.channels;
+    const avb::HostRect src = avb::host_rect(h_src, src_pitch, d.src_w * C, elem_size(d.in_type), wi.src_x0 * C,
+                                             wi.src_w * C, wi.src_y0, wi.src_h);
+    const avb::HostRect dst = avb::host_rect(h_dst, dst_pitch, w * C, elem_size(d.out_type), 0, w * C, 0, h);
+    const size_t ws = (size_t)h * wi.src_w * C * sizeof(float);
+    return avb::staged_call(pl->mx, pl->staging, pl->device, &pl->stream, src, dst, ws,
+                            [&](const void* s, void* o, void* wsp, cudaStream_t st) {
+                                return lancir_region(pl, x0, y0, w, h, wi.src_x0, wi.src_w, wi.src_y0, s, wi.src_w * C,
+                                                     o, w * C, wsp, st);
+                            });
 }
 
 } // extern "C"
@@ -912,15 +847,6 @@ namespace {
 int lshard_plan(const lancirb200_plan* pl, int rank, int nranks, avirb200_shard_info* si) {
     const lancirb200_plan_desc& d = pl->desc;
     return lshard(pl->pos_v.data(), pl->dv.kl, d.src_h, d.dst_h, rank, nranks, si);
-}
-
-int lgrow(void** p, size_t* have, size_t need) {
-    if (*have >= need) return 0;
-    cudaFree(*p);
-    *p = nullptr; *have = 0;
-    CUDA_TRY(cudaMalloc(p, need));
-    *have = need;
-    return 0;
 }
 
 // The exchange stream, forked from `st` (it starts after everything enqueued on st so far).
@@ -1125,41 +1051,16 @@ int lancirb200_resize_sharded_host(lancirb200_plan* pl, void* comm, int rank, in
     if (!pl || !h_src || !h_dst) return fail(AVIRB200_ERR_BAD_ARG, "null argument");
     const lancirb200_plan_desc& d = pl->desc;
     avirb200_shard_info si;
-    int r = lshard_plan(pl, rank, nranks, &si);
+    const int r = lshard_plan(pl, rank, nranks, &si);
     if (r != 0) return r;
-    if (src_pitch < (size_t)d.src_w * d.channels || dst_pitch < (size_t)d.dst_w * d.channels)
-        return fail(AVIRB200_ERR_BAD_ARG, "pitch smaller than a row");
-    const size_t in_el = elem_size(d.in_type), out_el = elem_size(d.out_type);
-    const size_t in_row = (size_t)d.src_w * d.channels * in_el, out_row = (size_t)d.dst_w * d.channels * out_el;
-    std::lock_guard<std::mutex> lk(pl->mx);
-    // the call runs on the plan's device; the caller's current device is restored on every exit
-    struct DeviceGuard {
-        int prev = -1;
-        ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
-    } guard;
-    {
-        int cur = -1;
-        CUDA_TRY(cudaGetDevice(&cur));
-        if (cur != pl->device) {
-            CUDA_TRY(cudaSetDevice(pl->device));
-            guard.prev = cur;
-        }
-    }
-    if (!pl->stream) CUDA_TRY(cudaStreamCreateWithFlags(&pl->stream, cudaStreamNonBlocking));
-    if ((r = lgrow(&pl->d_src, &pl->src_bytes, in_row * si.src_rows)) != 0 ||
-        (r = lgrow(&pl->d_dst, &pl->dst_bytes, out_row * si.dst_rows)) != 0 ||
-        (r = lgrow(&pl->d_ws, &pl->ws_bytes, LShardWs(d, si).total)) != 0)
-        return r;
-    CUDA_TRY(cudaMemcpy2DAsync(pl->d_src, in_row, h_src, src_pitch * in_el, in_row, si.src_rows, cudaMemcpyHostToDevice,
-                               pl->stream));
-    const size_t sp = (size_t)d.src_w * d.channels, dp = (size_t)d.dst_w * d.channels;
-    r = nranks == 1 ? lancirb200_resize_device(pl, pl->d_src, sp, pl->d_dst, dp, pl->d_ws, pl->stream)
-                    : lsharded(pl, comm, rank, nranks, pl->d_src, sp, pl->d_dst, dp, pl->d_ws, pl->stream);
-    if (r != 0) return r;
-    CUDA_TRY(cudaMemcpy2DAsync(h_dst, dst_pitch * out_el, pl->d_dst, out_row, out_row, si.dst_rows, cudaMemcpyDeviceToHost,
-                               pl->stream));
-    CUDA_TRY(cudaStreamSynchronize(pl->stream));
-    return 0;
+    const size_t sw = (size_t)d.src_w * d.channels, dw = (size_t)d.dst_w * d.channels;
+    const avb::HostRect src = avb::host_rect(h_src, src_pitch, sw, elem_size(d.in_type), 0, sw, 0, si.src_rows);
+    const avb::HostRect dst = avb::host_rect(h_dst, dst_pitch, dw, elem_size(d.out_type), 0, dw, 0, si.dst_rows);
+    return avb::staged_call(pl->mx, pl->staging, pl->device, &pl->stream, src, dst, LShardWs(d, si).total,
+                            [&](const void* s, void* o, void* w, cudaStream_t st) {
+                                return nranks == 1 ? lancirb200_resize_device(pl, s, sw, o, dw, w, st)
+                                                   : lsharded(pl, comm, rank, nranks, s, sw, o, dw, w, st);
+                            });
 }
 
 int lancirb200_resize_sharded_local(const lancirb200_plan* cpl, int nranks, const void* d_src, size_t src_pitch,

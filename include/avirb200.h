@@ -162,8 +162,17 @@ int avirb200_row_pass_device(const avirb200_plan* plan, const void* d_src, size_
 int avirb200_col_pass_device(const avirb200_plan* plan, const void* d_workspace, void* d_dst,
                              size_t dst_pitch, void* stream);
 
+/* HOST ENTRY POINTS (avirb200_resize_host, avirb200_resize_window_host, avirb200_resize_sharded_host and
+ * CLancIR's lancirb200_resize_host, _window_host and _sharded_host) share one contract.  Pitches are in
+ * elements; a pitch smaller than a row of the caller's image is AVIRB200_ERR_BAD_ARG before any CUDA call.
+ * The call runs on the plan's device, whichever device is current, and the caller's current device is
+ * unchanged afterwards.  It copies the caller's rows into device staging buffers, runs the device call on
+ * the plan's own stream, copies the result out and synchronises.  AVIR plans stage in buffers shared by
+ * every AVIR plan of the device, so AVIR host calls on one device run one at a time; a CLancIR plan stages
+ * in buffers of its own.  Host calls on one plan run one at a time.  Pageable or page-locked memory. */
+
 /* Convenience used by the drop-in resizeImage(): host buffers in, host buffers out
- * (H2D, both passes, D2H, synchronise).  Device buffers are cached inside the plan.
+ * (H2D, both passes, D2H, synchronise).
  * Images of 64 MiB and more are cut into row bands travelling on separate copy-in / compute /
  * copy-out streams, so that the PCIe transfers of both directions overlap each other and the
  * kernels (page-locked host memory lets them run asynchronously); the result bits do not
@@ -222,8 +231,8 @@ int avirb200_window_workspace_bytes(const avirb200_plan* plan, int x0, int y0, i
 int avirb200_resize_window_device(const avirb200_plan* plan, int x0, int y0, int w, int h, const void* d_src,
                                   size_t src_pitch, void* d_dst, size_t dst_pitch, void* d_workspace,
                                   void* stream);
-/* The same with HOST buffers: h_src is the WHOLE source image (only the footprint is copied to the
- * device), h_dst receives the w x h window.  Pageable or page-locked memory; synchronises. */
+/* The same with HOST buffers (a host entry point): h_src is the WHOLE source image (only the footprint is
+ * copied to the device), h_dst receives the w x h window. */
 int avirb200_resize_window_host(avirb200_plan* plan, int x0, int y0, int w, int h, const void* h_src,
                                 size_t src_pitch, void* h_dst, size_t dst_pitch);
 
@@ -307,9 +316,9 @@ int avirb200_resize_sharded(const avirb200_plan* plan, void* comm, int rank, int
                             const void* d_src, size_t src_pitch, void* d_dst, size_t dst_pitch,
                             void* d_workspace, void* stream);
 
-/* The same with HOST buffers (this rank's source band in, its destination band out): copies
- * in, avirb200_resize_sharded on the plan's own stream, copies out, synchronises.  Staging
- * buffers are cached in the plan.  The multi-GPU form of avirb200_resize_host. */
+/* The same with HOST buffers (a host entry point): this rank's source band in, its destination band
+ * out, through avirb200_resize_sharded on the plan's own stream.  The multi-GPU form of
+ * avirb200_resize_host. */
 int avirb200_resize_sharded_host(avirb200_plan* plan, void* comm, int rank, int nranks,
                                  const void* h_src, size_t src_pitch, void* h_dst, size_t dst_pitch);
 
@@ -362,8 +371,7 @@ void lancirb200_plan_destroy(lancirb200_plan* plan);
 int lancirb200_plan_workspace_bytes(const lancirb200_plan* plan, size_t* bytes);
 int lancirb200_resize_device(const lancirb200_plan* plan, const void* d_src, size_t src_pitch,
                              void* d_dst, size_t dst_pitch, void* d_workspace, void* stream);
-/* Host buffers in and out, on the plan's device; synchronises; the caller's current device is unchanged
- * afterwards. */
+/* Host buffers in and out (a host entry point, see avirb200_resize_host). */
 int lancirb200_resize_host(lancirb200_plan* plan, const void* h_src, size_t src_pitch,
                            void* h_dst, size_t dst_pitch);
 
@@ -392,9 +400,8 @@ int lancirb200_window_workspace_bytes(const lancirb200_plan* plan, int x0, int y
 int lancirb200_resize_window_device(const lancirb200_plan* plan, int x0, int y0, int w, int h, const void* d_src,
                                     size_t src_pitch, void* d_dst, size_t dst_pitch, void* d_workspace,
                                     void* stream);
-/* The same with HOST buffers: h_src is the WHOLE source image (only the footprint is copied to the
- * device), h_dst receives the w x h window.  Pageable or page-locked memory; synchronises; the
- * caller's current device is unchanged afterwards. */
+/* The same with HOST buffers (a host entry point, see avirb200_resize_host): h_src is the WHOLE source
+ * image (only the footprint is copied to the device), h_dst receives the w x h window. */
 int lancirb200_resize_window_host(lancirb200_plan* plan, int x0, int y0, int w, int h, const void* h_src,
                                   size_t src_pitch, void* h_dst, size_t dst_pitch);
 
@@ -426,9 +433,8 @@ int lancirb200_shard_workspace_bytes(const lancirb200_plan* plan, int rank, int 
  * exchanges with ncclSend / ncclRecv into the workspace's halo segments before the column pass. */
 int lancirb200_resize_sharded(const lancirb200_plan* plan, void* comm, int rank, int nranks, const void* d_src,
                               size_t src_pitch, void* d_dst, size_t dst_pitch, void* d_workspace, void* stream);
-/* The same with HOST buffers (this rank's source band in, its destination band out), staged through the
- * plan's buffers on the plan's stream, on the plan's device; synchronises; the caller's current device is
- * unchanged afterwards. */
+/* The same with HOST buffers (a host entry point, see avirb200_resize_host): this rank's source band in,
+ * its destination band out. */
 int lancirb200_resize_sharded_host(lancirb200_plan* plan, void* comm, int rank, int nranks, const void* h_src,
                                    size_t src_pitch, void* h_dst, size_t dst_pitch);
 /* Validation aid: every band of an `nranks` split on the CURRENT device, with full-image buffers.  The bands

@@ -18,7 +18,11 @@ that a later change to the routing predicates cannot quietly turn these into con
 """
 import contextlib
 import ctypes as C
+import json
+import os
 import re
+import subprocess
+import sys
 
 import numpy as np
 import pytest
@@ -30,6 +34,7 @@ import oracle_ref as o
 pytestmark = pytest.mark.gpu
 
 u8, u16, f32, f64 = np.uint8, np.uint16, np.float32, np.float64
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 TAIL = 64 << 10  # workspace guard bytes past what the library asked for
 FAMILIES = pytest.mark.parametrize("family", [0, 2, 1], ids=["product", "tile", "generic"])
 
@@ -479,7 +484,9 @@ ROUTES = [
 ]
 
 
-def test_layouts_route_to_the_kernels_they_cover():
+def route_failures():
+    """(case, layout, kernels launched, kernels wanted) of each call that runs other kernels than it is meant to
+    cover; None when the profiler records no kernel activity."""
     import torch
     failures = []
     for case, layout, family, want in ROUTES:
@@ -490,7 +497,7 @@ def test_layouts_route_to_the_kernels_they_cover():
             got = launched_kernels(lambda: _ok(L.avirb200_resize_device(
                 pl, dptr(d_src, sl), sl.pitch, dptr(d_dst, dl), dl.pitch, ws.data_ptr(), None)))
         if got is None:
-            pytest.skip("torch.profiler recorded no CUDA kernel activity on this machine")
+            return None
         if got != want:
             failures.append((cs.case_id(case), layout, family, got, want))
     for c in LANCIR_CASES[:1]:
@@ -518,4 +525,17 @@ def test_layouts_route_to_the_kernels_they_cover():
             if got != [col, row]:
                 failures.append(("lancir", layout, got, [col, row]))
     torch.cuda.synchronize()
+    return failures
+
+
+def test_layouts_route_to_the_kernels_they_cover():
+    """Run in a child process: a profiler session leaves state behind in the process that runs it, so that
+    whether this one records kernels would depend on which tests ran before it."""
+    code = ("import json, sys; sys.path[:0] = [%r, %r]; import test_gpu_layouts as t; "
+            "print(json.dumps(t.route_failures()))" % (ROOT, os.path.join(ROOT, "tests")))
+    r = subprocess.run([sys.executable, "-c", code], cwd=ROOT, capture_output=True, text=True, timeout=600)
+    assert r.returncode == 0, r.stderr[-4000:]
+    failures = json.loads(r.stdout.strip().splitlines()[-1])
+    if failures is None:
+        pytest.skip("torch.profiler recorded no CUDA kernel activity on this machine")
     assert not failures, failures

@@ -681,3 +681,31 @@ def test_host_calls_restore_the_callers_device():
     torch.cuda.set_device(0)
     assert cs.value_mismatch(outs[0][0], outs[1][0]) == 0
     assert cs.value_mismatch(crop(outs[0][0], win), outs[1][1]) == 0
+
+    # AVIR's three host calls (the sharded one as its single rank)
+    case = AVIR["tile"][0]
+    fp, sw, sh, nw, nh, ch, ti, to = case[:8]
+    src = cs.make_input(case, seed=91)
+    win = _window_of(nw, nh)
+    outs = {}
+    for dev in (0, 1):
+        torch.cuda.set_device(dev)
+        with avir_case("tile") as (L, pl, _):
+            L.avirb200_resize_sharded_host.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
+                                                       C.c_size_t, C.c_void_p, C.c_size_t]
+            torch.cuda.set_device(0)
+            assert current() == 0
+            full, band = np.zeros((nh, nw, ch), to), np.zeros((nh, nw, ch), to)
+            part = np.zeros((win[3], win[2], ch), to)
+            _ok(L.avirb200_resize_host(pl, src.ctypes.data, sw * ch, full.ctypes.data, nw * ch))
+            assert current() == 0, "avirb200_resize_host left device %d current" % current()
+            _ok(L.avirb200_resize_window_host(pl, *win, src.ctypes.data, sw * ch, part.ctypes.data, win[2] * ch))
+            assert current() == 0, "avirb200_resize_window_host left device %d current" % current()
+            _ok(L.avirb200_resize_sharded_host(pl, None, 0, 1, src.ctypes.data, sw * ch, band.ctypes.data, nw * ch))
+            assert current() == 0, "avirb200_resize_sharded_host left device %d current" % current()
+            outs[dev] = (full, part, band)
+            torch.cuda.set_device(dev)  # (the plan is destroyed on its own device)
+    torch.cuda.set_device(0)
+    assert cs.value_mismatch(outs[0][0], outs[1][0]) == 0
+    assert cs.value_mismatch(crop(outs[0][0], win), outs[1][1]) == 0
+    assert cs.value_mismatch(outs[0][0], outs[1][2]) == 0

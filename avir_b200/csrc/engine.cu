@@ -83,10 +83,6 @@ struct HostAxis {
 
 } // namespace
 
-namespace {
-struct Halo;
-}
-
 struct avirb200_plan {
     avirb200_plan_desc desc;     // in_type / out_type: what the KERNELS read and write (F64 -> F32)
     int io_in_type = 0, io_out_type = 0; // the caller's element types
@@ -121,9 +117,7 @@ struct avirb200_plan {
     int opt_overlap = 3;      // sharded: how the halo rows travel (AVIRB200_OPT_OVERLAP_HALO; 3 = fused into the kernels)
     int sm_count = 132;       // of `device`
     size_t smem_optin = 232448; // of `device`: the most dynamic shared memory one block may opt in to
-    Halo* halo = nullptr; // sharded: peer mailboxes (created by the first sharded call)
-    cudaStream_t stream_x = nullptr; // sharded: exchange stream
-    cudaEvent_t ev_x0 = nullptr, ev_x1 = nullptr;
+    PeerExchange x;           // sharded: the halo exchange (opened by the first sharded call of more than one rank)
 };
 
 namespace {
@@ -371,33 +365,12 @@ int run_pass(const avirb200_plan* pl, const PassRequest& req, cudaStream_t st, i
     return 0;
 }
 
+// The bands of rank `rank` of `nranks`; need_*: the intermediate rows its column pass reads.
 int shard_compute_axis(const DevAxis& vaxis, int rank, int nranks, avirb200_shard_info* info) {
-    if (nranks < 1 || rank < 0 || rank >= nranks) return fail(AVIRB200_ERR_BAD_ARG, "bad rank");
-    const int src_h = vaxis.src_len, dst_h = vaxis.dst_len;
-    auto src_split = [&](int r) { return (int)((long long)src_h * r / nranks); };
-    auto dst_split = [&](int r) { return (int)((long long)dst_h * r / nranks); };
-    info->src_row0 = src_split(rank);
-    info->src_rows = src_split(rank + 1) - info->src_row0;
-    info->dst_row0 = dst_split(rank);
-    info->dst_rows = dst_split(rank + 1) - info->dst_row0;
-    if (info->dst_rows <= 0 || info->src_rows <= 0)
-        return fail(AVIRB200_ERR_UNSUPPORTED, "image has fewer rows than ranks");
-    Range need = chain_source_range(vaxis,
-                                    Range{info->dst_row0, info->dst_row0 + info->dst_rows - 1},
-                                    nullptr);
-    // The band always contains the rank's own rows (they are produced locally anyway).
-    need.a = imin(need.a, info->src_row0);
-    need.b = imax(need.b, info->src_row0 + info->src_rows - 1);
-    info->need_row0 = need.a;
-    info->need_rows = need.b - need.a + 1;
-    info->halo_up = info->src_row0 - need.a;
-    info->halo_down = need.b - (info->src_row0 + info->src_rows - 1);
-    if (rank > 0 && info->halo_up > src_split(rank) - src_split(rank - 1))
-        return fail(AVIRB200_ERR_UNSUPPORTED, "halo exceeds the neighbouring band (too many ranks)");
-    if (rank + 1 < nranks && info->halo_down > src_split(rank + 2 > nranks ? nranks : rank + 2) -
-                                                   src_split(rank + 1))
-        return fail(AVIRB200_ERR_UNSUPPORTED, "halo exceeds the neighbouring band (too many ranks)");
-    return 0;
+    int r = shard_split(vaxis.src_len, vaxis.dst_len, rank, nranks, info);
+    if (r != 0) return r;
+    const Range need = chain_source_range(vaxis, Range{info->dst_row0, info->dst_row0 + info->dst_rows - 1}, nullptr);
+    return shard_halos(need.a, need.b + 1, vaxis.src_len, rank, nranks, info);
 }
 
 int shard_compute(const avirb200_plan* pl, int rank, int nranks, avirb200_shard_info* info) {
@@ -914,13 +887,6 @@ struct MailboxLayout {
     }
 };
 
-struct Halo : PeerBoxes { // (box: my mailbox; box_up / box_down: rank-1's and rank+1's, mapped)
-    void* comm = nullptr;
-    int rank = -1, nranks = 0;
-    MailboxLayout mine, above, below; // the layouts of the three
-    unsigned seq = 0;
-};
-
 // Waits for the neighbours' sequence numbers, then moves their rows from the mailbox into the
 // workspace (both directions, one launch).
 __global__ void __launch_bounds__(256) halo_pull_kernel(const volatile unsigned* flags, unsigned seq, int need_up,
@@ -983,54 +949,19 @@ __global__ void __launch_bounds__(256) lin2srgb_selftest_kernel(unsigned long lo
     atomicAdd(out + 1, bad);
 }
 
-void halo_free(Halo* h) {
-    if (h == nullptr) return;
-    peer_boxes_close(h);
-    delete h;
-}
-
-// Collective over `comm` (every rank of the sharded call makes it): builds and maps the mailboxes.
-// Leaves h->usable false (on EVERY rank) when any rank could not: the NCCL schedule runs then.
-int halo_setup(avirb200_plan* pl, void* comm, int rank, int nranks, cudaStream_t st) {
-    Nccl* nc = nccl();
-    if (!nc) return fail(AVIRB200_ERR_NCCL, "libnccl.so.2 not loadable");
-    halo_free(pl->halo);
-    Halo* h = pl->halo = new Halo();
-    h->comm = comm; h->rank = rank; h->nranks = nranks;
-    auto layout = [&](int q, MailboxLayout& l) -> int {
-        avirb200_shard_info si;
-        const int r = shard_compute(pl, q, nranks, &si);
-        if (r == 0) l = MailboxLayout(pl, si);
-        return r;
-    };
-    int r = layout(rank, h->mine);
-    if (r == 0 && rank > 0) r = layout(rank - 1, h->above);
-    if (r == 0 && rank + 1 < nranks) r = layout(rank + 1, h->below);
-    if (r != 0) return r;
-    return peer_boxes_open(comm, rank, nranks, h->mine.bytes(2), MailboxLayout::kHeader, st, h);
-}
-
 // Sharded calls: after the row pass (stream st) the band's boundary rows go to the neighbours' mailboxes on
-// the exchange stream (copy engines), each followed by the call's sequence number (at hs).
-int sharded_push(avirb200_plan* pl, cudaStream_t st, const float* own, const avs::StreamLink& l, const unsigned* hs) {
-    const size_t rowf = mid_pitch(pl);
+// the exchange stream (copy engines), each followed by the call's sequence number (at `word`).
+int sharded_push(avirb200_plan* pl, cudaStream_t st, const float* own, const avs::StreamLink& l, const unsigned* word) {
+    const size_t rowf = mid_pitch(pl), rowb = rowf * sizeof(float);
     const int top_rows = avs::stream_rows_up(l), bot_rows = avs::stream_rows_down(l);
-    if (pl->stream_x == nullptr) CUDA_TRY(cudaStreamCreateWithFlags(&pl->stream_x, cudaStreamNonBlocking));
-    if (pl->ev_x0 == nullptr) CUDA_TRY(cudaEventCreateWithFlags(&pl->ev_x0, cudaEventDisableTiming));
-    if (pl->ev_x1 == nullptr) CUDA_TRY(cudaEventCreateWithFlags(&pl->ev_x1, cudaEventDisableTiming));
-    CUDA_TRY(cudaEventRecord(pl->ev_x0, st));
-    CUDA_TRY(cudaStreamWaitEvent(pl->stream_x, pl->ev_x0, 0));
-    if (top_rows > 0) {
-        CUDA_TRY(cudaMemcpyAsync(l.above.from_dn, own, (size_t)top_rows * rowf * 4, cudaMemcpyDefault, pl->stream_x));
-        CUDA_TRY(cudaMemcpyAsync(&l.above.flags[1], hs, 4, cudaMemcpyDefault, pl->stream_x));
-    }
-    if (bot_rows > 0) {
-        CUDA_TRY(cudaMemcpyAsync(l.below.from_up, own + (size_t)(l.me->src_rows - bot_rows) * rowf,
-                                 (size_t)bot_rows * rowf * 4, cudaMemcpyDefault, pl->stream_x));
-        CUDA_TRY(cudaMemcpyAsync(&l.below.flags[0], hs, 4, cudaMemcpyDefault, pl->stream_x));
-    }
-    CUDA_TRY(cudaEventRecord(pl->ev_x1, pl->stream_x));
-    return 0;
+    PeerExchange& x = pl->x;
+    int r = x.fork(st);
+    if (r == 0 && top_rows > 0)
+        r = push_rows(l.above.from_dn, rowb, own, rowb, rowb, top_rows, &l.above.flags[1], word, x.stream);
+    if (r == 0 && bot_rows > 0)
+        r = push_rows(l.below.from_up, rowb, own + (size_t)(l.me->src_rows - bot_rows) * rowf, rowb, rowb, bot_rows,
+                      &l.below.flags[0], word, x.stream);
+    return r;
 }
 
 // Plans the banded host call runs unbanded: double buffers and error diffusion (bands on one compute stream would
@@ -1242,10 +1173,7 @@ void avirb200_plan_destroy(avirb200_plan* pl) {
     if (pl == nullptr) return;
     cudaFree(pl->arena);
     fast_plan_free(pl->fast);
-    halo_free(pl->halo);
-    if (pl->stream_x) cudaStreamDestroy(pl->stream_x);
-    if (pl->ev_x0) cudaEventDestroy(pl->ev_x0);
-    if (pl->ev_x1) cudaEventDestroy(pl->ev_x1);
+    pl->x.close();
     if (pl->stream) cudaStreamDestroy(pl->stream);
     if (pl->stream_in) cudaStreamDestroy(pl->stream_in);
     if (pl->stream_out) cudaStreamDestroy(pl->stream_out);
@@ -1279,11 +1207,7 @@ int resize_region(const avirb200_plan* pl, const avirb200_window_info* win, int 
     const int src_w = win ? win->src_w : d.src_w, src_h = win ? win->src_h : d.src_h;
     if (src_pitch < (size_t)src_w * d.channels || dst_pitch < (size_t)w * d.channels)
         return fail(AVIRB200_ERR_BAD_ARG, "pitch smaller than a row");
-    {
-        int cur = -1;
-        if (cudaGetDevice(&cur) != cudaSuccess || cur != pl->device)
-            return fail(AVIRB200_ERR_BAD_ARG, "the current device is not the plan's device");
-    }
+    if (const int e = check_device(pl->device)) return e;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     int launches = 0;
     char* wsb = static_cast<char*>(d_ws);
@@ -1666,27 +1590,6 @@ int avirb200_shard_layout_desc(const avirb200_plan_desc* desc, int rank, int nra
     return 0;
 }
 
-int avirb200_comm_unique_id(void* id128) {
-    Nccl* nc = nccl();
-    if (!nc) return fail(AVIRB200_ERR_NCCL, "libnccl.so.2 not loadable");
-    NCCL_TRY(nc->GetUniqueId(id128));
-    return 0;
-}
-
-int avirb200_comm_create(const void* id128, int rank, int nranks, void** comm_out) {
-    Nccl* nc = nccl();
-    if (!nc) return fail(AVIRB200_ERR_NCCL, "libnccl.so.2 not loadable");
-    Id128 id;
-    std::memcpy(&id, id128, sizeof id);
-    NCCL_TRY(nc->CommInitRank(comm_out, nranks, id, rank));
-    return 0;
-}
-
-void avirb200_comm_destroy(void* comm) {
-    Nccl* nc = nccl();
-    if (nc && nc->CommDestroy && comm) nc->CommDestroy(comm);
-}
-
 } // extern "C"
 
 namespace {
@@ -1694,9 +1597,10 @@ namespace {
 // avirb200_resize_sharded; for nranks > 1 the caller holds pl->mx.
 int sharded(avirb200_plan* pl, void* comm, int rank, int nranks, const void* d_src, size_t src_pitch, void* d_dst,
             size_t dst_pitch, void* d_ws, cudaStream_t st) {
-    { int cur = -1; if (cudaGetDevice(&cur) != cudaSuccess || cur != pl->device) return fail(AVIRB200_ERR_BAD_ARG, "the current device is not the plan's device"); }
+    int r = check_device(pl->device);
+    if (r != 0) return r;
     avirb200_shard_info si;
-    int r = shard_compute(pl, rank, nranks, &si);
+    r = shard_compute(pl, rank, nranks, &si);
     if (r != 0) return r;
     const avirb200_plan_desc& d = pl->desc;
     const size_t rowf = mid_pitch(pl);
@@ -1739,9 +1643,8 @@ int sharded(avirb200_plan* pl, void* comm, int rank, int nranks, const void* d_s
         pl->last_launches.store(launches, std::memory_order_relaxed);
         return r;
     }
-    if (comm == nullptr) return fail(AVIRB200_ERR_BAD_ARG, "sharded resize needs a communicator");
-    Nccl* nc = nccl();
-    if (!nc) return fail(AVIRB200_ERR_NCCL, "libnccl.so.2 not loadable");
+    Nccl* nc = nullptr;
+    if ((r = comm_nccl(comm, &nc)) != 0) return r;
     // What the neighbours need from this rank is symmetric information: compute theirs.
     avirb200_shard_info up, down;
     std::memset(&up, 0, sizeof up); std::memset(&down, 0, sizeof down);
@@ -1753,18 +1656,11 @@ int sharded(avirb200_plan* pl, void* comm, int rank, int nranks, const void* d_s
     link.dn = (rank + 1 < nranks) ? &down : nullptr;
     const int top_rows = avs::stream_rows_up(link), bot_rows = avs::stream_rows_down(link);
 
-    if (pl->opt_overlap) {
-        if (pl->halo == nullptr || pl->halo->comm != comm || pl->halo->rank != rank || pl->halo->nranks != nranks) {
-            r = halo_setup(pl, comm, rank, nranks, st); // collective, once per plan
-            if (r != 0) return r;
-        }
-    }
-    Halo* h = (pl->opt_overlap && pl->halo && pl->halo->usable) ? pl->halo : nullptr;
-    if (h != nullptr) {
-        const unsigned seq = ++h->seq;
-        const int slot = (int)(seq & 1u);
-        unsigned* hs = &h->h_seq[seq & 63u];
-        *hs = seq;
+    PeerExchange& x = pl->x;
+    const MailboxLayout mine(pl, si), above(pl, up), below(pl, down);
+    if (pl->opt_overlap && (r = x.open(comm, rank, nranks, mine.bytes(2), MailboxLayout::kHeader, st)) != 0) return r;
+    if (pl->opt_overlap && x.usable) {
+        const PeerExchange::Call call = x.next_call();
         const char* srcb = static_cast<const char*>(d_src);
         auto rows_pass = [&](int row0, int nrows) -> int {
             PassRequest q = row_request(d, srcb + (size_t)row0 * src_pitch * in_el, src_pitch, nrows,
@@ -1774,10 +1670,10 @@ int sharded(avirb200_plan* pl, void* comm, int rank, int nranks, const void* d_s
         };
         const int need_up = (link.up && si.halo_up > 0) ? 1 : 0;
         const int need_down = (link.dn && si.halo_down > 0) ? 1 : 0;
-        link.seq = seq;
-        link.mine = h->mine.at(h->box, slot);
-        if (link.up) link.above = h->above.at(h->box_up, slot);
-        if (link.dn) link.below = h->below.at(h->box_down, slot);
+        link.seq = call.seq;
+        link.mine = mine.at(x.box, call.slot);
+        if (link.up) link.above = above.at(x.box_up, call.slot);
+        if (link.dn) link.below = below.at(x.box_down, call.slot);
         // AVIRB200_OPT_OVERLAP_HALO = 3, the fused exchange: the row kernel stores the rows the neighbours need
         // into their mailboxes as it produces them (peer stores over NVLink) and raises their flags when the
         // last of them is out; the column kernel reads the neighbours' rows in place from this rank's mailbox,
@@ -1793,7 +1689,7 @@ int sharded(avirb200_plan* pl, void* comm, int rank, int nranks, const void* d_s
             if (send) q.link = &link;
             if ((r = run_pass(pl, q, st, &launches)) != 0) return r;
             if (!send) { // (not on the streaming kernel: the copy engines push)
-                if ((r = sharded_push(pl, st, own, link, hs)) != 0) return r;
+                if ((r = sharded_push(pl, st, own, link, call.word)) != 0) return r;
                 pushed = true;
             }
         } else {
@@ -1813,7 +1709,7 @@ int sharded(avirb200_plan* pl, void* comm, int rank, int nranks, const void* d_s
             } else if ((r = run_pass(pl, row, st, &launches)) != 0) {
                 return r;
             }
-            if ((r = sharded_push(pl, st, own, link, hs)) != 0) return r;
+            if ((r = sharded_push(pl, st, own, link, call.word)) != 0) return r;
             pushed = true;
             if (split && (r = rows_pass(top_rows, si.src_rows - top_rows - bot_rows)) != 0) return r;
         }
@@ -1826,12 +1722,12 @@ int sharded(avirb200_plan* pl, void* comm, int rank, int nranks, const void* d_s
         } else {
             if (need_up || need_down) {
                 (void)cudaGetLastError();
-                halo_pull_kernel<<<64, 256, 0, st>>>(link.mine.flags, seq, need_up, need_down,
+                halo_pull_kernel<<<64, 256, 0, st>>>(link.mine.flags, call.seq, need_up, need_down,
                                                      reinterpret_cast<const float4*>(link.mine.from_up), reinterpret_cast<float4*>(mid),
-                                                     need_up ? h->mine.up_bytes / 16 : 0,
+                                                     need_up ? mine.up_bytes / 16 : 0,
                                                      reinterpret_cast<const float4*>(link.mine.from_dn),
                                                      reinterpret_cast<float4*>(own + (size_t)si.src_rows * rowf),
-                                                     need_down ? h->mine.down_bytes / 16 : 0);
+                                                     need_down ? mine.down_bytes / 16 : 0);
                 ++launches;
                 CUDA_TRY(cudaGetLastError());
             }
@@ -1844,14 +1740,14 @@ int sharded(avirb200_plan* pl, void* comm, int rank, int nranks, const void* d_s
         // needs no rows from below (halo_down 0) has no such wait: its D row goes through NCCL instead.
         if (r == 0 && f32_out) {
             ErrdCarry cy;
-            cy.seq = seq;
+            cy.seq = call.seq;
             float* carry = reinterpret_cast<float*>(wsb + ws.errd_carry);
             const size_t rowd = (size_t)d.dst_w * d.channels;
             const bool in_box = link.up && up.halo_down > 0, out_box = link.dn && si.halo_down > 0;
             if (pl->errd && link.up) {
                 if (in_box) {
-                    cy.in = h->mine.errd_row(h->box, slot);
-                    cy.in_prog = h->mine.errd_progress(h->box, slot);
+                    cy.in = mine.errd_row(x.box, call.slot);
+                    cy.in_prog = mine.errd_progress(x.box, call.slot);
                 } else {
                     NCCL_TRY(nc->Recv(carry, rowd, 7, rank - 1, comm, st));
                     cy.in = carry;
@@ -1859,8 +1755,8 @@ int sharded(avirb200_plan* pl, void* comm, int rank, int nranks, const void* d_s
             }
             if (pl->errd && link.dn) {
                 if (out_box) {
-                    cy.out = h->below.errd_row(h->box_down, slot);
-                    cy.out_prog = h->below.errd_progress(h->box_down, slot);
+                    cy.out = below.errd_row(x.box_down, call.slot);
+                    cy.out_prog = below.errd_progress(x.box_down, call.slot);
                 } else {
                     cy.out = carry + rowd;
                 }
@@ -1869,7 +1765,7 @@ int sharded(avirb200_plan* pl, void* comm, int rank, int nranks, const void* d_s
             if (r == 0 && pl->errd && link.dn && !out_box) NCCL_TRY(nc->Send(cy.out, rowd, 7, rank + 1, comm, st));
         }
         // the pushes read this call's workspace: the caller's stream does not end before them
-        if (pushed) CUDA_TRY(cudaStreamWaitEvent(st, pl->ev_x1, 0));
+        if (const int e = pushed ? x.join(st) : 0) return e;
         pl->last_launches.store(launches, std::memory_order_relaxed);
         return r;
     }

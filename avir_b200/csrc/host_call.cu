@@ -51,6 +51,13 @@ HostRect host_rect(const void* img, size_t pitch, size_t line, size_t el, size_t
     return r;
 }
 
+int check_device(int device) {
+    int cur = -1;
+    if (cudaGetDevice(&cur) != cudaSuccess || cur != device)
+        return fail(AVIRB200_ERR_BAD_ARG, "the current device is not the plan's device");
+    return 0;
+}
+
 DeviceScope::~DeviceScope() {
     if (prev_ >= 0) cudaSetDevice(prev_);
 }

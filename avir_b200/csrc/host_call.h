@@ -40,6 +40,10 @@ struct HostRect {
 // elements apart, in elements of `el` bytes.
 HostRect host_rect(const void* img, size_t pitch, size_t line, size_t el, size_t x, size_t w, int y, int rows);
 
+// AVIRB200_ERR_BAD_ARG unless `device` is current: the device entry points run on their plan's device, which the
+// caller makes current.
+int check_device(int device);
+
 // Makes a device current for its lifetime; the device that was current before is current again afterwards.
 class DeviceScope {
 public:

@@ -481,28 +481,12 @@ int lwindow(const int32_t* hpos, int hkl, const int32_t* vpos, int vkl, int src_
 // destination rows dst_h * r / n).  need_* are SOURCE rows: the band's vertical footprint (lspan) joined with
 // its own source band; the halos are the rows of it beyond the band, which the neighbours hold.
 int lshard(const int32_t* vpos, int vkl, int src_h, int dst_h, int rank, int nranks, avirb200_shard_info* info) {
-    if (nranks < 1 || rank < 0 || rank >= nranks) return fail(AVIRB200_ERR_BAD_ARG, "bad rank");
-    auto src_split = [&](int r) { return (int)((long long)src_h * r / nranks); };
-    auto dst_split = [&](int r) { return (int)((long long)dst_h * r / nranks); };
-    info->src_row0 = src_split(rank);
-    info->src_rows = src_split(rank + 1) - info->src_row0;
-    info->dst_row0 = dst_split(rank);
-    info->dst_rows = dst_split(rank + 1) - info->dst_row0;
-    if (info->dst_rows <= 0 || info->src_rows <= 0) return fail(AVIRB200_ERR_UNSUPPORTED, "image has fewer rows than ranks");
+    const int r = avb::shard_split(src_h, dst_h, rank, nranks, info);
+    if (r != 0) return r;
     if (info->dst_rows > 65535) return fail(AVIRB200_ERR_UNSUPPORTED, "band too tall (more than 65535 destination rows)");
     int32_t lo = 0, n = 0;
     lspan(vpos, vkl, src_h, info->dst_row0, info->dst_rows, &lo, &n);
-    const int a = lo < info->src_row0 ? lo : info->src_row0;
-    const int b = lo + n > info->src_row0 + info->src_rows ? lo + n : info->src_row0 + info->src_rows;
-    info->need_row0 = a;
-    info->need_rows = b - a;
-    info->halo_up = info->src_row0 - a;
-    info->halo_down = b - (info->src_row0 + info->src_rows);
-    if (rank > 0 && info->halo_up > info->src_row0 - src_split(rank - 1))
-        return fail(AVIRB200_ERR_UNSUPPORTED, "halo exceeds the neighbouring band (too many ranks)");
-    if (rank + 1 < nranks && info->halo_down > src_split(rank + 2) - src_split(rank + 1))
-        return fail(AVIRB200_ERR_UNSUPPORTED, "halo exceeds the neighbouring band (too many ranks)");
-    return 0;
+    return avb::shard_halos(lo, lo + n, src_h, rank, nranks, info);
 }
 
 // Bytes of one source row in a halo segment: 16-byte aligned, so that the vector kernel's loads stay aligned.
@@ -541,13 +525,6 @@ struct LBoxLayout {
     char* from_down(char* box, int slot) const { return from_up(box, slot) + avb::align_up(up_bytes, 256); }
 };
 
-struct LHalo : avb::PeerBoxes {
-    void* comm = nullptr;
-    int rank = -1, nranks = 0;
-    LBoxLayout mine, above, below;
-    unsigned seq = 0;
-};
-
 } // namespace
 
 struct lancirb200_plan {
@@ -561,10 +538,7 @@ struct lancirb200_plan {
     cudaStream_t stream = nullptr;
     // row-sharded calls
     int opt_overlap = 3;           // AVIRB200_OPT_OVERLAP_HALO: 3 mailboxes, 0 NCCL
-    LHalo* halo = nullptr;         // the peer mailboxes (created by the first sharded call)
-    unsigned* h_one = nullptr;     // pinned 1: the flag value of lancirb200_resize_sharded_local
-    cudaStream_t stream_x = nullptr; // exchange stream
-    cudaEvent_t ev_x0 = nullptr, ev_x1 = nullptr;
+    avb::PeerExchange x;           // the halo exchange (opened by the first sharded call of more than one rank)
 };
 
 extern "C" {
@@ -633,14 +607,7 @@ void lancirb200_plan_destroy(lancirb200_plan* pl) {
     if (!pl) return;
     cudaFree(pl->arena);
     if (pl->stream) cudaStreamDestroy(pl->stream);
-    if (pl->halo) {
-        avb::peer_boxes_close(pl->halo);
-        delete pl->halo;
-    }
-    cudaFreeHost(pl->h_one);
-    if (pl->stream_x) cudaStreamDestroy(pl->stream_x);
-    if (pl->ev_x0) cudaEventDestroy(pl->ev_x0);
-    if (pl->ev_x1) cudaEventDestroy(pl->ev_x1);
+    pl->x.close();
     delete pl;
 }
 
@@ -849,23 +816,14 @@ int lshard_plan(const lancirb200_plan* pl, int rank, int nranks, avirb200_shard_
     return lshard(pl->pos_v.data(), pl->dv.kl, d.src_h, d.dst_h, rank, nranks, si);
 }
 
-// The exchange stream, forked from `st` (it starts after everything enqueued on st so far).
-int lfork(lancirb200_plan* pl, cudaStream_t st) {
-    if (pl->stream_x == nullptr) CUDA_TRY(cudaStreamCreateWithFlags(&pl->stream_x, cudaStreamNonBlocking));
-    if (pl->ev_x0 == nullptr) CUDA_TRY(cudaEventCreateWithFlags(&pl->ev_x0, cudaEventDisableTiming));
-    if (pl->ev_x1 == nullptr) CUDA_TRY(cudaEventCreateWithFlags(&pl->ev_x1, cudaEventDisableTiming));
-    CUDA_TRY(cudaEventRecord(pl->ev_x0, st));
-    CUDA_TRY(cudaStreamWaitEvent(pl->stream_x, pl->ev_x0, 0));
-    return 0;
-}
-
-// `n` source rows of a band from its row `r0` into a halo segment (rows lhalo_row_bytes apart), on `st`.
-int lcopy_rows(const lancirb200_plan* pl, void* seg, const void* band, size_t src_pitch, int r0, int n, cudaStream_t st) {
+// `n` source rows of a band from its row `r0` into a halo segment (rows lhalo_row_bytes apart) on `st`, then,
+// when `flag` is given, the 4-byte `word` into it.
+int lpush_rows(const lancirb200_plan* pl, void* seg, const void* band, size_t src_pitch, int r0, int n, void* flag,
+               const unsigned* word, cudaStream_t st) {
     const lancirb200_plan_desc& d = pl->desc;
     const size_t el = elem_size(d.in_type);
-    CUDA_TRY(cudaMemcpy2DAsync(seg, lhalo_row_bytes(d), static_cast<const char*>(band) + (size_t)r0 * src_pitch * el,
-                               src_pitch * el, (size_t)d.src_w * d.channels * el, n, cudaMemcpyDefault, st));
-    return 0;
+    return avb::push_rows(seg, lhalo_row_bytes(d), static_cast<const char*>(band) + (size_t)r0 * src_pitch * el,
+                          src_pitch * el, (size_t)d.src_w * d.channels * el, n, flag, word, st);
 }
 
 // A band's passes: the column pass over its segmented source (s: the segments, flags and sequence number),
@@ -900,10 +858,7 @@ int lcheck(const lancirb200_plan* pl, size_t src_pitch, size_t dst_pitch) {
     const lancirb200_plan_desc& d = pl->desc;
     if (src_pitch < (size_t)d.src_w * d.channels || dst_pitch < (size_t)d.dst_w * d.channels)
         return fail(AVIRB200_ERR_BAD_ARG, "pitch smaller than a row");
-    int cur = -1;
-    if (cudaGetDevice(&cur) != cudaSuccess || cur != pl->device)
-        return fail(AVIRB200_ERR_BAD_ARG, "the current device is not the plan's device");
-    return 0;
+    return avb::check_device(pl->device);
 }
 
 // lancirb200_resize_sharded for nranks > 1; the caller holds pl->mx.
@@ -917,26 +872,16 @@ int lsharded(lancirb200_plan* pl, void* comm, int rank, int nranks, const void* 
     if (r == 0 && rank > 0) r = lshard_plan(pl, rank - 1, nranks, &up);
     if (r == 0 && rank + 1 < nranks) r = lshard_plan(pl, rank + 1, nranks, &dn);
     if (r != 0) return r;
-    if (comm == nullptr) return fail(AVIRB200_ERR_BAD_ARG, "sharded resize needs a communicator");
-    avb::Nccl* nc = avb::nccl();
-    if (!nc) return fail(AVIRB200_ERR_NCCL, "libnccl.so.2 not loadable");
-    if (pl->opt_overlap && (!pl->halo || pl->halo->comm != comm || pl->halo->rank != rank || pl->halo->nranks != nranks)) {
-        if (pl->halo) {
-            avb::peer_boxes_close(pl->halo);
-            delete pl->halo;
-        }
-        LHalo* h = pl->halo = new LHalo(); // collective, once per plan
-        h->comm = comm; h->rank = rank; h->nranks = nranks;
-        h->mine = LBoxLayout(d, si);
-        h->above = LBoxLayout(d, up);
-        h->below = LBoxLayout(d, dn);
-        if ((r = avb::peer_boxes_open(comm, rank, nranks, h->mine.bytes(2), LBoxLayout::kHeader, st, h)) != 0) return r;
-    }
-    LHalo* h = (pl->opt_overlap && pl->halo && pl->halo->usable) ? pl->halo : nullptr;
+    avb::Nccl* nc = nullptr;
+    if ((r = avb::comm_nccl(comm, &nc)) != 0) return r;
+    avb::PeerExchange& x = pl->x;
+    const LBoxLayout mine(d, si), above(d, up), below(d, dn);
+    if (pl->opt_overlap && (r = x.open(comm, rank, nranks, mine.bytes(2), LBoxLayout::kHeader, st)) != 0) return r;
     // A pair of neighbours exchanges through the mailboxes when rows travel both ways (DESIGN.md section 7: then
     // neither can run two calls ahead of the other); otherwise, and on the NCCL schedule, through NCCL.
-    const bool box_up = h && rank > 0 && si.halo_up > 0 && up.halo_down > 0;
-    const bool box_dn = h && rank + 1 < nranks && si.halo_down > 0 && dn.halo_up > 0;
+    const bool boxes = pl->opt_overlap && x.usable;
+    const bool box_up = boxes && rank > 0 && si.halo_up > 0 && up.halo_down > 0;
+    const bool box_dn = boxes && rank + 1 < nranks && si.halo_down > 0 && dn.halo_up > 0;
     const bool nccl_up = !box_up && rank > 0 && (si.halo_up > 0 || up.halo_down > 0);
     const bool nccl_dn = !box_dn && rank + 1 < nranks && (si.halo_down > 0 || dn.halo_up > 0);
     const LShardWs wl(d, si);
@@ -952,28 +897,23 @@ int lsharded(lancirb200_plan* pl, void* comm, int rank, int nranks, const void* 
         // the rows each neighbour needs go into its mailbox (this call's slot) on the exchange stream, each
         // direction followed by the call's sequence number in the neighbour's flag; no kernel of this call
         // comes before them
-        const unsigned seq = ++h->seq;
-        const int slot = (int)(seq & 1u);
-        unsigned* hs = &h->h_seq[seq & 63u];
-        *hs = seq;
-        s.seq = seq;
-        if ((r = lfork(pl, st)) != 0) return r;
+        const avb::PeerExchange::Call call = x.next_call();
+        s.seq = call.seq;
+        if ((r = x.fork(st)) != 0) return r;
         if (box_up) {
-            if ((r = lcopy_rows(pl, h->above.from_down(h->box_up, slot), d_src, src_pitch, 0, up.halo_down, pl->stream_x)) != 0)
+            if ((r = lpush_rows(pl, above.from_down(x.box_up, call.slot), d_src, src_pitch, 0, up.halo_down, x.box_up + 4,
+                                call.word, x.stream)) != 0)
                 return r;
-            CUDA_TRY(cudaMemcpyAsync(h->box_up + 4, hs, 4, cudaMemcpyDefault, pl->stream_x));
-            s.up = h->mine.from_up(h->box, slot);
-            s.flag_up = reinterpret_cast<const volatile unsigned*>(h->box);
+            s.up = mine.from_up(x.box, call.slot);
+            s.flag_up = reinterpret_cast<const volatile unsigned*>(x.box);
         }
         if (box_dn) {
-            if ((r = lcopy_rows(pl, h->below.from_up(h->box_down, slot), d_src, src_pitch, si.src_rows - dn.halo_up,
-                                dn.halo_up, pl->stream_x)) != 0)
+            if ((r = lpush_rows(pl, below.from_up(x.box_down, call.slot), d_src, src_pitch, si.src_rows - dn.halo_up,
+                                dn.halo_up, x.box_down, call.word, x.stream)) != 0)
                 return r;
-            CUDA_TRY(cudaMemcpyAsync(h->box_down, hs, 4, cudaMemcpyDefault, pl->stream_x));
-            s.dn = h->mine.from_down(h->box, slot);
-            s.flag_dn = reinterpret_cast<const volatile unsigned*>(h->box + 4);
+            s.dn = mine.from_down(x.box, call.slot);
+            s.flag_dn = reinterpret_cast<const volatile unsigned*>(x.box + 4);
         }
-        CUDA_TRY(cudaEventRecord(pl->ev_x1, pl->stream_x));
         pushed = true;
     }
     // the other pairs: one message per row into the workspace's halo segments, grouped before the column pass
@@ -994,7 +934,7 @@ int lsharded(lancirb200_plan* pl, void* comm, int rank, int nranks, const void* 
     }
     r = lband(pl, si, d_src, src_pitch, d_dst, dst_pitch, d_ws, s, st);
     // the pushes read the caller's source band: the caller's stream does not end before them
-    if (pushed) CUDA_TRY(cudaStreamWaitEvent(st, pl->ev_x1, 0));
+    if (const int e = pushed ? x.join(st) : 0) return e;
     return r;
 }
 
@@ -1091,29 +1031,25 @@ int lancirb200_resize_sharded_local(const lancirb200_plan* cpl, int nranks, cons
     // column kernel waiting on the flags.  On the NCCL schedule (AVIRB200_OPT_OVERLAP_HALO = 0) the rows are
     // copied into the same segments before the column passes, which then do not wait.
     const bool box = pl->opt_overlap != 0 && nranks > 1;
+    avb::PeerExchange& x = pl->x;
     cudaStream_t sx = st;
     if (box) {
-        if (!pl->h_one) {
-            CUDA_TRY(cudaHostAlloc(&pl->h_one, sizeof(unsigned), cudaHostAllocPortable));
-            *pl->h_one = 1;
-        }
+        if ((e = x.pin()) != 0) return e;
         for (int r = 0; r < nranks; ++r) CUDA_TRY(cudaMemsetAsync(ws[r] + wl[r].header, 0, 8, st));
-        if ((e = lfork(pl, st)) != 0) return e;
-        sx = pl->stream_x;
+        if ((e = x.fork(st)) != 0) return e;
+        sx = x.stream;
     }
+    const unsigned* one = box ? x.one() : nullptr;
     for (int r = 0; r < nranks; ++r) {
         const avirb200_shard_info& b = si[r];
-        if (b.halo_up > 0) { // band r-1's last rows
-            if ((e = lcopy_rows(pl, ws[r] + wl[r].up, srcb, src_pitch, b.need_row0, b.halo_up, sx)) != 0) return e;
-            if (box) CUDA_TRY(cudaMemcpyAsync(ws[r] + wl[r].header, pl->h_one, 4, cudaMemcpyDefault, sx));
-        }
-        if (b.halo_down > 0) { // band r+1's first rows
-            if ((e = lcopy_rows(pl, ws[r] + wl[r].down, srcb, src_pitch, b.src_row0 + b.src_rows, b.halo_down, sx)) != 0)
-                return e;
-            if (box) CUDA_TRY(cudaMemcpyAsync(ws[r] + wl[r].header + 4, pl->h_one, 4, cudaMemcpyDefault, sx));
-        }
+        char* flags = box ? ws[r] + wl[r].header : nullptr;
+        // band r-1's last rows, then band r+1's first rows
+        if (b.halo_up > 0 && (e = lpush_rows(pl, ws[r] + wl[r].up, srcb, src_pitch, b.need_row0, b.halo_up, flags, one, sx)) != 0)
+            return e;
+        if (b.halo_down > 0 && (e = lpush_rows(pl, ws[r] + wl[r].down, srcb, src_pitch, b.src_row0 + b.src_rows, b.halo_down,
+                                               flags ? flags + 4 : nullptr, one, sx)) != 0)
+            return e;
     }
-    if (box) CUDA_TRY(cudaEventRecord(pl->ev_x1, sx));
     int r = 0;
     for (int q = 0; q < nranks && r == 0; ++q) {
         const avirb200_shard_info& b = si[q];
@@ -1129,7 +1065,7 @@ int lancirb200_resize_sharded_local(const lancirb200_plan* cpl, int nranks, cons
         r = lband(pl, b, srcb + (size_t)b.src_row0 * src_pitch * in_el, src_pitch,
                   static_cast<char*>(d_dst) + (size_t)b.dst_row0 * dst_pitch * out_el, dst_pitch, ws[q], s, st);
     }
-    if (box) CUDA_TRY(cudaStreamWaitEvent(st, pl->ev_x1, 0));
+    if (box && (e = x.join(st)) != 0) return e;
     return r;
 }
 
